@@ -75,7 +75,8 @@ constexpr int DF_OFF_BB = DF_OFF_SCAN + 256 * 4;             /* u32[512] code-bu
 constexpr int DF_OFF_MISC = DF_OFF_BB + 512 * 4;             /* u32[32] + mbarrier */
 constexpr int DF_OFF_SINK = DF_OFF_MISC + 32 * 4 + 16;       /* u32[32]: one word per lane, the target of atomics that have nothing to do
                                                               * (ptxas branches around a predicated ATOMS; a select on the address is one instruction) */
-constexpr int DF_SMEM_BYTES = DF_OFF_SINK + 32 * 4;
+constexpr int DF_OFF_LSYM = DF_OFF_SINK + 32 * 4;            /* u16[256]: length - 3 -> length symbol (0..28) | extra value << 5; filled once per CTA */
+constexpr int DF_SMEM_BYTES = DF_OFF_LSYM + 256 * 2;
 constexpr uint32_t DF_ZERO_SYM = 286;                        /* literal/length symbol that never occurs: its table entries are all zero */
 static_assert(DF_HASH_ENTRIES * 4 <= DF_STAGE_WORDS * 4, "hash fits the staging region");
 /* The history variant (template parameter HIST, levels 6-9): the previous 32 KiB -- the chunk's first unit, or with DF_FLAG_DICT the
@@ -136,6 +137,11 @@ __device__ __forceinline__ void dist_symbol0(uint32_t d, uint32_t &sym, uint32_t
 }
 __device__ __forceinline__ uint32_t len_extra_bits(uint32_t lsym) { return (lsym < 8 || lsym >= 28) ? 0u : (lsym >> 2) - 1; }
 __device__ __forceinline__ uint32_t dist_extra_bits(uint32_t dsym) { return dsym < 4 ? 0u : (dsym >> 1) - 1; }
+
+/* byte address of the staging word that holds bit `pos`, from the region base: pos >> 5 by a high multiply, so that both steps run
+ * on the FMA pipe (a shift and a mask would be two integer-ALU instructions; the emit pass is bound by that pipe). The bit offset in
+ * the word needs no mask either where it feeds a funnel shift, which takes the amount modulo 32. */
+__device__ __forceinline__ uint32_t stage_word(uint32_t base, uint32_t pos, uint32_t k4) { return base + __umulhi(pos, 1u << 27) * k4; }
 
 /* OR `n` (<=32) bits of v into the staging bit string at bit position pos */
 __device__ __forceinline__ void stage_put(uint32_t *stage, uint32_t pos, uint32_t v, uint32_t n) {
@@ -453,9 +459,16 @@ __device__ __forceinline__ uint32_t extend_match8(const Smem &sm, uint32_t c, ui
     return len < maxlen ? len : maxlen;
 }
 
+/* The constant 4 as a value the compiler cannot see (the kernel always runs DF_THREADS threads per CTA): an address `i * k4 + base`
+ * stays one IMAD on the FMA pipe, where `i * 4 + base` would become a LEA on the integer-ALU pipe -- the pipe this kernel is bound
+ * by. (A constant behind an inline-asm mov would not do: ptxas folds it.) */
+__device__ __forceinline__ uint32_t opaque4() { return blockDim.x / (uint32_t)(DF_THREADS / 4); }
+
 template <bool HIST>
-__device__ __forceinline__ uint32_t hash_addr(uint32_t v) { /* byte offset of the key of 4-byte value v */
-    return (HIST ? DFH_OFF_HASH : DF_OFF_HASH) + (((v * 2654435761u) >> (32 - (HIST ? DFH_HASH_BITS : DF_HASH_BITS))) << 2);
+__device__ __forceinline__ uint32_t hash_addr(uint32_t v, uint32_t k4) { /* byte offset of the key of 4-byte value v; k4 = opaque4() */
+    /* the top bits of v * 2654435761 by a high multiply, then * 4: all on the FMA pipe (a shift and a mask would be two integer-ALU
+     * instructions) */
+    return (HIST ? DFH_OFF_HASH : DF_OFF_HASH) + __umulhi(v * 2654435761u, 1u << (HIST ? DFH_HASH_BITS : DF_HASH_BITS)) * k4;
 }
 
 /* span record (two words, parked in the token region during the parse):
@@ -479,18 +492,21 @@ __device__ __forceinline__ void span_classify(const Smem &sm, uint32_t A, uint32
     const uint32_t crel = cover > q0 ? cover - q0 : 0u;
     const uint32_t cr8 = crel < 8 ? crel : 8u;
     uint32_t ex = 0;
-    uint32_t M[2] = {0, 0};
+    MA = MB = 0; /* (scalars, not an array: an array of two ends up in local memory) */
 #pragma unroll
     for (int r = 0; r < (ONEM ? 1 : 2); r++) {
+        /* The match keeps what lies at or behind s = max(start, cover): Lf = end - s bytes, none when the cover reaches its end
+         * (an empty record has end = start). Kept whole (s = start) it has at least 4; trimmed, 3 or more stay a match (ordered
+         * at the cover's slot, min(s, 8) & 7) and 1 or 2 become the leftover literals. */
         const uint32_t R = r == 0 ? A : B;
-        const uint32_t L = rec_len(R), j = R & 7u, end = j + L;
-        const bool kept = L != 0 && j >= crel;
-        const bool strad = L != 0 && j < crel && end > crel;
-        const uint32_t rem = end - crel;
-        const uint32_t Lf = kept ? L : ((strad && rem >= 3) ? rem : 0u);
-        const uint32_t d1 = (R >> 11) & 0x7fffu;
-        M[r] = Lf ? (0x80000000u | ((kept ? j : cr8) & 7u) | ((Lf - 3) << 4) | (d1 << 12)) : 0u;
-        ex = (strad && rem < 3) ? rem : ex;
+        const uint32_t j = R & 7u, end = j + rec_len(R);
+        const uint32_t s = j > crel ? j : crel;
+        const uint32_t Lf = (end > s ? end : s) - s;
+        const uint32_t P = (s < 8u ? s : 8u) & 7u;
+        const uint32_t M = Lf >= 3 ? (((Lf << 4) + (0x80000000u - (3u << 4))) | P | ((R << 1) & (0x7fffu << 12))) : 0u;
+        if (r == 0) MA = M;
+        else MB = M;
+        ex = Lf - 1u < 2u ? Lf : ex;
     }
     F = ((lit >> cr8) << cr8) | (ex << 8);
     if (ex) { /* rare: fetch the leftover bytes now, the write pass then needs nothing but F */
@@ -498,21 +514,19 @@ __device__ __forceinline__ void span_classify(const Smem &sm, uint32_t A, uint32
         F |= sm.ld8(p) << 16;
         if (ex == 2) F |= sm.ld8(p + 1) << 24;
     }
-    MA = M[0];
-    MB = M[1];
 }
 
 /* final match record (P | len | dist form) -> symbol form, counting its two symbols on the way:
  *   bit 31 valid | P << 28 (3 bits; 8 -> 0: then the span has no literals, so the order does not matter)
  *   | distance extra value << 15 (13 bits) | distance symbol << 10 | length extra value << 5 | length symbol (0..28) */
 __device__ __forceinline__ uint32_t match_symbols(const Smem &sm, uint32_t M) {
-    uint32_t ls, lb, lv, ds, db;
-    length_symbol(fin_len(M), ls, lb, lv);
+    uint32_t ds, db;
+    const uint32_t lsv = sm.ld16(DF_OFF_LSYM + ((M >> 3) & 0x1feu)); /* length symbol | extra value << 5, by length - 3 */
     const uint32_t d = fin_dist(M) - 1;
     dist_symbol0(d, ds, db);
-    sm.red_add32(DF_OFF_HIST + (257u + ls) * 4, 1u);
+    sm.red_add32(DF_OFF_HIST + (257u + (lsv & 31u)) * 4, 1u);
     sm.red_add32(DF_OFF_HIST + (288u + ds) * 4, 1u);
-    return 0x80000000u | ((M & 7u) << 28) | ((d & ((1u << db) - 1u)) << 15) | (ds << 10) | (lv << 5) | ls;
+    return 0x80000000u | ((M & 7u) << 28) | ((d & ((1u << db) - 1u)) << 15) | (ds << 10) | lsv;
 }
 /* bits a match costs (both code words with their extra bits); 0 for an empty record */
 __device__ __forceinline__ uint32_t match_bits(const Smem &sm, uint32_t M) {
@@ -528,9 +542,9 @@ __device__ __forceinline__ void put_match_bits(const Smem &sm, uint32_t pos, uin
     const uint32_t n1 = cl + ((cwl >> 20) & 15u);
     const uint32_t v2 = (cwd & 0x7fffu) | (((M >> 15) & 0x1fffu) << cd);     /* <= 15 + 13 bits */
     const uint64_t V = (uint64_t)v1 | ((uint64_t)v2 << n1);
-    const uint32_t lo = (uint32_t)V, hi = (uint32_t)(V >> 32), sh = pos & 31u;
-    const uint32_t wa = DF_OFF_STAGE + (pos >> 5) * 4;
-    const uint32_t w0 = lo << sh, w1 = __funnelshift_l(lo, hi, sh), w2 = __funnelshift_l(hi, 0u, sh);
+    const uint32_t lo = (uint32_t)V, hi = (uint32_t)(V >> 32);
+    const uint32_t wa = stage_word(DF_OFF_STAGE, pos, opaque4());
+    const uint32_t w0 = __funnelshift_l(0u, lo, pos), w1 = __funnelshift_l(lo, hi, pos), w2 = __funnelshift_l(hi, 0u, pos);
     sm.red_or32(wa, w0);
     sm.red_or32(wa + 4, w1);
     if (w2) sm.red_or32(wa + 8, w2);
@@ -560,6 +574,30 @@ __device__ __forceinline__ uint32_t nth_parked(const uint32_t (&bm)[DF_NBATCH], 
     }
     return found ? bsel * (uint32_t)DF_THREADS + warp * 32u + base : 0xffffffffu;
 }
+
+/* ---- opt-in per-phase cycle counters (compile with -DMZ_DF_PHASES: `make phases`, read by tools/deflate_phases.py) ---------------
+ * Thread 0 of every CTA reads clock64() right after the barrier that ends a phase and adds the cycles since its previous reading to
+ * column `phase` of the CTA's row of g_df_phases (column DF_PH_UNITS counts the units). After a barrier every thread of the CTA is
+ * done with the phase before, so the deltas are the CTA's wall time per phase; no barrier is added. Without the macro (the product
+ * library) and on the emulator the marks compile to nothing. */
+enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_E_SCAN, DF_PH_F_M3, DF_PH_FLUSH, DF_PH_UNITS, DF_PH_COLS };
+constexpr int DF_PH_ROWS = 1024;
+#if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
+__device__ unsigned long long g_df_phases[DF_PH_ROWS][DF_PH_COLS];
+#define DF_PHASE_BEGIN(t) unsigned long long t = clock64()
+#define DF_PHASE(t, ph)                                                                        \
+    do {                                                                                       \
+        if (threadIdx.x == 0 && blockIdx.x < (unsigned)DF_PH_ROWS) {                           \
+            const unsigned long long now_ = clock64();                                         \
+            atomicAdd(&g_df_phases[blockIdx.x][ph], now_ - (t));                               \
+            if ((ph) == DF_PH_LOAD) atomicAdd(&g_df_phases[blockIdx.x][DF_PH_UNITS], 1ull);   \
+            (t) = now_;                                                                        \
+        }                                                                                      \
+    } while (0)
+#else
+#define DF_PHASE_BEGIN(t)
+#define DF_PHASE(t, ph)
+#endif
 
 /* ---- the kernel ------------------------------------------------------------------------------- */
 template <int STRIDE, bool LAZY, bool HIST = false>
@@ -593,10 +631,16 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
     const unsigned lane = lane_id(), warp = warp_id();
     Smem sm;
     sm.init(smem);
+    if (tid < 256) { /* the length-symbol table (read first in the classify pass of the first unit, many barriers later) */
+        uint32_t ls, lb, lv;
+        length_symbol(tid + 3, ls, lb, lv);
+        sm.st16(DF_OFF_LSYM + tid * 2, ls | (lv << 5));
+    }
     /* ONEM = keep only the first match of a span (a second one becomes literals): every later phase then carries one match
      * record per span instead of two. Measured on the emulator: 3 % larger output on text at stride 2 (short matches are
      * common), so it is off; the switch stays for experiments. */
     constexpr bool ONEM = false;
+    DF_PHASE_BEGIN(ph_t); /* (the chunk's set-up counts to the load of its first unit, its trailer to the flush of its last) */
 
     /* Chunks are handed out by an atomic counter: if another kernel holds some SMs, the resident CTAs simply
      * take more chunks instead of leaving a tail to late CTAs. */
@@ -721,11 +765,12 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
                         const uint32_t v = j == 0 ? x.x : (j < 4 ? __funnelshift_r(x.x, x.y, 8 * j) : (j == 4 ? x.y : __funnelshift_r(x.y, y, 8 * (j - 4))));
-                        sm.red_min32(hash_addr<true>(v), key0 + j);
+                        sm.red_min32(hash_addr<true>(v, 4u), key0 + j);
                     }
                 }
                 __syncthreads();
             }
+            DF_PHASE(ph_t, DF_PH_LOAD);
 
             uint32_t fF[DF_NBATCH], fA[DF_NBATCH];
             bool stored = (P.level == 0);
@@ -738,6 +783,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 for (uint32_t b = 0; b < nb; b++) {
                     const uint32_t q0 = b * DF_BATCH + tid * DF_SPAN;
                     uint32_t v[12], ha[8], lc[8];
+                    const uint32_t k4 = opaque4();
                     {
                         const uint2 x = sm.ld64(DF_OFF_IN + q0), y = sm.ld64(DF_OFF_IN + q0 + 8);
                         v[0] = x.x; v[4] = x.y; v[8] = y.x;
@@ -750,7 +796,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     }
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
-                        ha[j] = hash_addr<HIST>(v[j]);
+                        ha[j] = hash_addr<HIST>(v[j], k4);
                         if (j % STRIDE == 0) lc[j] = sm.ld32(ha[j]); /* key of the latest earlier batch that holds this hash */
                     }
                     const uint32_t nvalid = ulen > q0 ? (ulen - q0 < 8 ? ulen - q0 : 8u) : 0u;
@@ -795,25 +841,53 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     /* ---- W: walk the span: static and branch-free. A match whose lockstep length is the cap (8) reaches the end of
                      * the span whatever its true length is, so it is always the span's last token: it is extended once, after
                      * the walk ------------------------------------------------------------------------------------------------ */
-                    uint32_t nxt = 0, lit = 0, mA = 0, mB = 0;
+                    uint32_t nxt = 0, lit = 0, mA = 0, mB = 0, span_end = 0;
+                    if (STRIDE == 2 && !LAZY && !ONEM) {
+                        /* Level 1: candidates only at even positions, lengths 0 or >= 4. The walk then takes the first even position
+                         * with a match (A: before it, and after its end, every position is a literal until the next even one), and
+                         * then the first even position at or behind A's end that has one (B, which runs past the span). The same
+                         * tokens as the walk below, as two chains of selects and two masks. */
+                        uint32_t endA = 0, endB = 0;
 #pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const bool take = nxt == (uint32_t)j;
-                        if (j % STRIDE == 0) {
+                        for (int j = 6; j >= 0; j -= 2) {
                             const uint32_t l = lc[j] & 15u;
-                            bool ism = take && l >= (uint32_t)DF_MINMATCH;
-                            if (LAZY && STRIDE == 1 && j < 7) ism = ism && !((lc[j + 1] & 15u) > l);
                             const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
-                            const bool first = mA == 0;
-                            if (ONEM) ism = ism && first;
-                            mA = (ism && first) ? rec : mA;
-                            if (!ONEM) mB = (ism && !first) ? rec : mB;
-                            lit |= (take && !ism) ? (1u << j) : 0u;
-                            nxt = ism ? (uint32_t)j + l : (take ? (uint32_t)j + 1u : nxt);
-                        } else {
-                            lit |= take ? (1u << j) : 0u;
-                            nxt = take ? (uint32_t)j + 1u : nxt;
+                            mA = l ? rec : mA;
+                            endA = l ? (uint32_t)j + l : endA;
                         }
+#pragma unroll
+                        for (int j = 6; j >= 2; j -= 2) {
+                            const uint32_t l = lc[j] & 15u;
+                            const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
+                            const bool nextm = l != 0 && (uint32_t)j >= endA;
+                            mB = nextm ? rec : mB;
+                            endB = nextm ? (uint32_t)j + l : endB;
+                        }
+                        /* positions under no match are literals (no match: end = start = 0) */
+                        lit = ~(((1u << endA) - (1u << (mA & 7u))) | ((1u << endB) - (1u << (mB & 7u)))) & 0xffu;
+                        span_end = mB ? endB : endA;
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < 8; j++) {
+                            const bool take = nxt == (uint32_t)j;
+                            if (j % STRIDE == 0) {
+                                const uint32_t l = lc[j] & 15u;
+                                bool ism = take && l >= (uint32_t)DF_MINMATCH;
+                                if (LAZY && STRIDE == 1 && j < 7) ism = ism && !((lc[j + 1] & 15u) > l);
+                                const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
+                                const bool first = mA == 0;
+                                if (ONEM) ism = ism && first;
+                                mA = (ism && first) ? rec : mA;
+                                if (!ONEM) mB = (ism && !first) ? rec : mB;
+                                lit |= (take && !ism) ? (1u << j) : 0u;
+                                nxt = ism ? (uint32_t)j + l : (take ? (uint32_t)j + 1u : nxt);
+                            } else {
+                                lit |= take ? (1u << j) : 0u;
+                                nxt = take ? (uint32_t)j + 1u : nxt;
+                            }
+                        }
+                        const uint32_t last = mB ? mB : mA;
+                        span_end = last ? (last & 7u) + rec_len(last) : 0u;
                     }
                     lit &= (1u << nvalid) - 1u;
                     {
@@ -823,10 +897,11 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                         const uint32_t capped = __ballot_sync(MZ_FULL_MASK, ((last >> 3) & 255u) == (uint32_t)(DF_LOCKLEN - 3));
                         if (lane == 0) s_scan[b * DF_WARPS + warp] = capped;
                         sm.st64(DF_OFF_REC + (b * DF_THREADS + tid) * 8, mA | ((lit & 63u) << 26), mB | ((lit >> 6) << 26));
-                        /* start offset and end (relative to the span) of the span's last match */
-                        sm.st16(DF_OFF_SPN + (b * DF_THREADS + tid) * 2, last ? ((last & 7u) << 9) | ((last & 7u) + rec_len(last)) : 0u);
+                        /* start offset and end (relative to the span) of the span's last match (0 for none) */
+                        sm.st16(DF_OFF_SPN + (b * DF_THREADS + tid) * 2, ((last & 7u) << 9) | span_end);
                     }
                 }
+                DF_PHASE(ph_t, DF_PH_PARSE); /* (no barrier behind the last batch: warp 0's view; the walks left are uniform work) */
                 /* ---- M0: true lengths of the capped matches ----------------------------------------------------------------- */
                 {
                     __syncwarp();
@@ -898,6 +973,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     }
                 }
                 __syncthreads(); /* S1: records visible; the hash table is dead */
+                DF_PHASE(ph_t, DF_PH_M0);
 
                 /* ---- staging := 0 (+ the carried tail), histograms := 0 ------------------------------ */
                 for (uint32_t i = tid; i < DF_STAGE_WORDS / 4; i += DF_THREADS) {
@@ -962,12 +1038,14 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     *(uint4 *)(smem + DF_OFF_SPN + tid * 16) = make_uint4(cv[0] | (cv[1] << 16), cv[2] | (cv[3] << 16), cv[4] | (cv[5] << 16), cv[6] | (cv[7] << 16));
                 }
                 __syncthreads(); /* S3: covers visible */
+                DF_PHASE(ph_t, DF_PH_COVER);
 
                 /* ---- T: classify every span once -> final records; symbol counts. The first match of a span is turned into symbol
                  * form here (36 % of the spans have one); the second one (7 %) would keep the whole warp busy for two or three
                  * lanes, so it is parked in the record region (word 1 of the span's record, dead once it has been read) and the
                  * warp's ballots remember where: the M1 pass below works through them 32 at a time. -------------------------- */
                 const uint32_t hist_lit = sm.addr((lane & 1u) ? (uint32_t)DF_OFF_HIST2 : (uint32_t)DF_OFF_HIST); /* two copies halve the same-address traffic */
+                const uint32_t k4 = opaque4();
                 const uint32_t sink = sm.addr(DF_OFF_SINK + lane * 4);
                 uint32_t bmB[DF_NBATCH]; /* per batch: the lanes of this warp whose span has a second match (warp-uniform) */
 #pragma unroll
@@ -989,7 +1067,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
 #pragma unroll
                         for (int j = 0; j < 8; j++) {
                             const uint32_t by = MZ_BYTE(j < 4 ? x.x : x.y, j & 3);
-                            sm.red_add32_a(((F >> j) & 1u) ? by * 4u + hist_lit : sink, 1u);
+                            sm.red_add32_a(((F >> j) & 1u) ? by * k4 + hist_lit : sink, 1u);
                         }
                         if (MA) MA = match_symbols(sm, MA);
                         if (!ONEM) {
@@ -1015,14 +1093,16 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 }
                 if (tid == 0) sm.red_add32(DF_OFF_HIST + 256 * 4, 1u); /* end of block */
                 __syncthreads(); /* S4 */
+                DF_PHASE(ph_t, DF_PH_T_M1);
                 /* ---- D: codes (10 warps on a named barrier; the rest wait here) ------------------------- */
                 if (tid < DF_BB_THREADS)
                     block_build_codes(s_hist_ll, (const uint32_t *)(smem + DF_OFF_HIST2), s_hist_d, s_lens_ll, s_lens_d, s_code_ll, s_code_d, s_bits_ll, s_bits_d, s_bb,
                                       s_stage, bitpos, bfinal);
                 __syncthreads(); /* S5 */
+                DF_PHASE(ph_t, DF_PH_D);
                 const uint32_t hdrbits = s_bb[BB_HDRBITS]; /* (the scratch is reused below) */
                 /* ---- E: bits per span -> offsets ------------------------------------------------------------------- */
-                const uint32_t bits_base = sm.addr(DF_OFF_BITS);
+                const uint32_t bits_base = sm.addr(DF_OFF_BITS), zero_bits = sm.addr(DF_OFF_BITS + DF_ZERO_SYM);
 #pragma unroll
                 for (int b = 0; b < DF_NBATCH; b++) {
                     if ((uint32_t)b < nb) {
@@ -1035,8 +1115,9 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                         nbits += ex == 2 ? sm.ld8(DF_OFF_BITS + (F >> 24)) : 0u;
 #pragma unroll
                         for (int j = 0; j < 8; j++) {
-                            const uint32_t l = sm.ld8_a(bits_base + MZ_BYTE(j < 4 ? x.x : x.y, j & 3));
-                            nbits += ((F >> j) & 1u) ? l : 0u;
+                            /* a position that is not a literal reads the all-zero entry (like the emit pass: a select on the address, no
+                             * select on the value) */
+                            nbits += sm.ld8_a(((F >> j) & 1u) ? bits_base + MZ_BYTE(j < 4 ? x.x : x.y, j & 3) : zero_bits);
                         }
                         sm.st16(DF_OFF_SPN + sidx * 2, nbits);
                     }
@@ -1060,6 +1141,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     s_bb[tid] = mybase;
                 }
                 __syncthreads(); /* S9: offsets visible */
+                DF_PHASE(ph_t, DF_PH_E_SCAN);
                 const uint32_t eob = s_code_ll[256];
                 const uint32_t dyn_bits = hdrbits + tokbits + ((eob >> 16) & 15u);
                 const uint32_t stored_bits = (((bitpos + 3 + 7) & ~7u) - bitpos) + 32 + ulen * 8;
@@ -1080,6 +1162,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                      * one's position is parked next to its record for the M3 pass. ------------------------------------------- */
                     const uint32_t base = bitpos + hdrbits;
                     const uint32_t code_base = sm.addr(DF_OFF_CODE), zero_ent = sm.addr(DF_OFF_CODE + DF_ZERO_SYM * 4), stage_base = sm.addr(DF_OFF_STAGE);
+                    const uint32_t k4 = opaque4();
 #pragma unroll
                     for (int b = 0; b < DF_NBATCH; b++) {
                         if ((uint32_t)b < nb) {
@@ -1103,7 +1186,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
 #pragma unroll
                             for (int j = 0; j < 8; j++) {
                                 const uint32_t by = MZ_BYTE(j < 4 ? x.x : x.y, j & 3);
-                                cw[j] = sm.ld32_a(((F >> j) & 1u) ? by * 4u + code_base : zero_ent); /* code | length << 16 (a literal's entry has no extra-bits field) */
+                                cw[j] = sm.ld32_a(((F >> j) & 1u) ? by * k4 + code_base : zero_ent); /* code | length << 16 (a literal's entry has no extra-bits field) */
                             }
                             /* lengths, one per byte; a match leaves a gap of its size at its slot (slot 8 = none: the shifts clamp to 0) */
                             const uint32_t nA = match_bits(sm, MA), nB = ONEM ? 0u : match_bits(sm, MB);
@@ -1116,12 +1199,12 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
 #pragma unroll
                             for (int jj = 0; jj < 4; jj++) {
                                 const uint32_t pp = pos + MZ_BYTE(jj < 2 ? E0 : E1, 2 * (jj & 1));
-                                const uint32_t c0 = cw[2 * jj], c1 = cw[2 * jj + 1];
                                 /* at most the two literals are in-band, and then they are adjacent (a match start covers its neighbour) */
+                                const uint32_t c0 = cw[2 * jj], c1 = cw[2 * jj + 1];
                                 const uint32_t v = (c0 & 0xffffu) | ((c1 & 0xffffu) << (c0 >> 16));
-                                const uint32_t sh = pp & 31u, wa = stage_base + ((pp >> 5) << 2);
-                                sm.red_or32_a(wa, v << sh);
-                                sm.red_or32_a(wa + 4, __funnelshift_l(v, 0u, sh));
+                                const uint32_t wa = stage_word(stage_base, pp, k4);
+                                sm.red_or32_a(wa, __funnelshift_l(0u, v, pp));
+                                sm.red_or32_a(wa + 4, __funnelshift_l(v, 0u, pp));
                             }
                             if (MA) put_match_bits(sm, pos + (shr_clamp(E0, sA) & 0xffu) + (shr_clamp(E1, sA - 32u) & 0xffu), MA);
                             if (!ONEM) sm.st32(DF_OFF_REC + sidx * 8, pos + (shr_clamp(E0, sB) & 0xffu) + (shr_clamp(E1, sB - 32u) & 0xffu)); /* (only read back where MB != 0) */
@@ -1168,6 +1251,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 bitpos = (p0 + 4 + ulen) * 8;
             }
             __syncthreads();
+            DF_PHASE(ph_t, DF_PH_F_M3); /* (a stored block counts here) */
             /* ---- G: flush whole 16-byte units, carry the tail ------------------------------------ */
             {
                 const uint32_t n16 = bitpos >> 7;
@@ -1179,6 +1263,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 if (HIST && u + 1 < nunits) /* this unit is the next one's history */
                     for (uint32_t i = tid; i < (uint32_t)DF_UNIT / 16; i += DF_THREADS) *(uint4 *)(smem - DFH_PREV + i * 16) = *(const uint4 *)(s_in + i * 16);
                 __syncthreads();
+                DF_PHASE(ph_t, DF_PH_FLUSH);
             }
         }
 
@@ -1204,6 +1289,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
             if (tid < 8) ((uint32_t *)(gout + flushed))[tid] = s_stage[tid];
             if (tid == 0) P.out_len[chunk] = flushed + (bitpos >> 3);
             __syncthreads();
+            DF_PHASE(ph_t, DF_PH_FLUSH);
         }
     }
 }

@@ -384,6 +384,22 @@ int32_t mz_cuda_deflate_chunks(const void *d_in, uint64_t total_len, uint32_t ch
     return MZ_OK;
 }
 
+#if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
+/* Only in the instrumented library (`make phases`): copy the deflate kernel's per-CTA phase counters, `rows` rows of DF_PH_COLS
+ * u64 each (at most DF_PH_ROWS), to host memory and zero them on the device. Synchronises the device. */
+int32_t mz_cuda_deflate_phases(uint64_t *host, uint32_t rows) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!host || rows > (uint32_t)DF_PH_ROWS) return MZ_PARAM_ERROR;
+    static unsigned long long zero[DF_PH_ROWS][DF_PH_COLS];
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpyFromSymbol(host, g_df_phases, (size_t)rows * DF_PH_COLS * sizeof(uint64_t)));
+    CK(cudaMemcpyToSymbol(g_df_phases, zero, sizeof(zero)));
+    return MZ_OK;
+}
+#endif
+
 int32_t mz_cuda_concat(const void *d_slots, uint64_t slot_stride, const uint32_t *d_out_len, uint32_t nchunks, uint64_t *d_offsets,
                        void *d_dst, void *stream) {
     DeviceCtx *c;

@@ -1,0 +1,108 @@
+#!/usr/bin/env python3
+"""Where the deflate kernel's cycles go, per phase, on the GPU: runs the instrumented library (minizip-ng_b200/
+libmz_strm_cuda_phases.so, built by `make -C minizip-ng_b200/csrc phases`: deflate_kernel.cuh with -DMZ_DF_PHASES) on the bench
+text with the C5 launch (64 KiB chunks, one launch over the whole buffer, 2 CTAs per SM) and prints SM cycles per 32 KiB unit
+and each phase's share, with the GPU's name, power limit and SM clock.
+
+The counters are thread 0's clock64() readings at the kernel's barriers, summed per CTA; cycles per unit = all CTAs' cycles over
+all units. The counting itself costs a few atomics per unit, so the kernel time printed here is not the product's.
+  python tools/deflate_phases.py [--gib 2] [--level 1] [--reps 3] [--json OUT]"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+PHASES = ["load + hash reset", "parse batches", "M0", "cover", "T + M1", "D (codes + header)", "E + scan", "F + M3", "flush"]
+COLS = len(PHASES) + 1  # + units
+ROWS = 1024
+
+
+def gpu_info():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", "0"], stdout=subprocess.PIPE, text=True, timeout=30)
+        return dict(zip(q.split(","), [s.strip() for s in r.stdout.strip().split(",")]))
+    except (OSError, subprocess.SubprocessError):
+        return {}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--gib", type=float, default=2.0)
+    ap.add_argument("--level", type=int, default=1)
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+
+    import torch
+    import __graft_entry__ as ge
+    import textgen
+    path = os.path.join(ROOT, "minizip-ng_b200", "libmz_strm_cuda_phases.so")
+    if not os.path.exists(path):
+        sys.exit("%s is missing: make -C minizip-ng_b200/csrc phases" % path)
+    pkg = ge._load_pkg()
+    lib = pkg.configure(C.CDLL(path))
+    lib.mz_cuda_deflate_phases.restype = C.c_int32
+    lib.mz_cuda_deflate_phases.argtypes = [C.c_void_p, C.c_uint32]
+    torch.cuda.set_device(0)
+    pkg.check(lib.mz_cuda_init(), "mz_cuda_init")
+
+    chunk = 65536
+    n = int(args.gib * (1 << 30)) // chunk * chunk
+    nch = n // chunk
+    src = torch.empty(n, dtype=torch.uint8, device="cuda")
+    seg = 64 << 20
+    for o in range(0, n, seg):  # the bench's text: one seed per 64 MiB segment
+        textgen.device_into(src.data_ptr() + o, min(seg, n - o), 1000 + o // seg)
+    stride = int(lib.mz_cuda_deflate_slot_bound(chunk))
+    slots = torch.empty(nch * stride, dtype=torch.uint8, device="cuda")
+    out_len = torch.empty(nch, dtype=torch.int32, device="cuda")
+    rows = (C.c_uint64 * (ROWS * COLS))()
+
+    def launch():
+        pkg.check(lib.mz_cuda_deflate_chunks(src.data_ptr(), n, chunk, None, None, None, nch, pkg.FLAG_FINAL, args.level, slots.data_ptr(),
+                                             stride, out_len.data_ptr(), pkg._stream_ptr()), "deflate")
+
+    launch()  # warm-up
+    pkg.check(lib.mz_cuda_deflate_phases(rows, ROWS), "phases")
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    for _ in range(args.reps):
+        launch()
+    ev1.record()
+    torch.cuda.synchronize()
+    info = gpu_info()  # right after the timed launches (the clock it reports is the current one)
+    kms = ev0.elapsed_time(ev1) / args.reps
+    pkg.check(lib.mz_cuda_deflate_phases(rows, ROWS), "phases")
+    tab = [[rows[r * COLS + c] for c in range(COLS)] for r in range(ROWS)]
+    tab = [r for r in tab if r[-1]]
+    units = sum(r[-1] for r in tab)
+    per = [sum(r[c] for r in tab) for c in range(len(PHASES))]
+    total = sum(per)
+    busiest = max(sum(r[:-1]) for r in tab) / args.reps  # a CTA's cycles over the launch ~ kernel time x SM clock
+    res = {"gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock_after": info.get("clocks.sm"),
+           "sm_clock_max": info.get("clocks.max.sm"), "level": args.level, "bytes": n, "ctas": len(tab), "units": units // args.reps,
+           "kernel_ms": round(kms, 3), "input_GBps": round(n / kms / 1e6, 1), "effective_sm_MHz": round(busiest / (kms * 1e3), 0),
+           "ratio": round(int(out_len.sum().item()) / n, 4), "cycles_per_unit": round(total / units, 0),
+           "phases": {p: {"cycles_per_unit": round(c / units, 0), "share": round(c / total, 4)} for p, c in zip(PHASES, per)}}
+    print("%s, power limit %s, SM clock %s (max %s); effective clock during the launches %d MHz" % (
+        res["gpu"], res["power_limit"], res["sm_clock_after"], res["sm_clock_max"], res["effective_sm_MHz"]))
+    print("level %d, %.2f GiB of bench text, 64 KiB chunks, %d CTAs, %d units: %.3f ms per launch (instrumented), ratio %.4f" % (
+        args.level, n / (1 << 30), res["ctas"], res["units"], kms, res["ratio"]))
+    print("%-20s %12s %7s" % ("phase", "cycles/unit", "share"))
+    for p, c in zip(PHASES, per):
+        print("%-20s %12.0f %6.1f%%" % (p, c / units, 100.0 * c / total))
+    print("%-20s %12.0f" % ("total", total / units))
+    print(json.dumps(res))
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
