@@ -30,7 +30,7 @@ constexpr int CRC_THREADS = 1024;
 constexpr int CRC_ROW = 512;
 constexpr int CRC_TABLE_WORDS = 4 * 256 * 32; /* 128 KiB */
 constexpr int CRC_SMEM_BYTES = CRC_TABLE_WORDS * 4;
-constexpr int CRC_UNROLL = 4;
+constexpr int CRC_UNROLL = 4; /* rows per load batch; the next batch is in flight while one is folded */
 
 /* a(x) * b(x) mod P in the reflected representation (bit 31 = x^0). 32 shift-xor steps. */
 __host__ __device__ inline uint32_t gf2_mulmod(uint32_t a, uint32_t b) {
@@ -40,6 +40,12 @@ __host__ __device__ inline uint32_t gf2_mulmod(uint32_t a, uint32_t b) {
         b = (b >> 1) ^ (CRC_POLY & (0u - (b & 1u)));
     }
     return p;
+}
+
+/* a(x) * x^32 mod P: 32 multiplications by x */
+__host__ __device__ inline uint32_t gf2_mul_x32(uint32_t a) {
+    for (int i = 0; i < 32; i++) a = (a >> 1) ^ (CRC_POLY & (0u - (a & 1u)));
+    return a;
 }
 
 /* x^(2^k) mod P for k = 0..63, filled on the host once (crc_consts) */
@@ -76,16 +82,26 @@ struct CrcParams {
     const CrcConsts *consts; /* device copy */
     uint32_t *out_residue;   /* R(segment), per segment */
     uint32_t *out_crc;       /* optional: finalized crc32(0, segment) per segment */
+    uint64_t init_len;       /* 0, or a segment length whose init term ~0 * x^(8 init_len) the caller computed once: init */
+    uint32_t init;
 };
 
-#define MZ_CRC_STEP(s, w) \
-    (s) = t0[((s) & 0xffu) << 5] ^ t1[(((s) >> 8) & 0xffu) << 5] ^ t2[(((s) >> 16) & 0xffu) << 5] ^ t3[((s) >> 24) << 5] ^ (w)
+/* the init term of crc32(0, .) over len bytes, ~0 * x^(8 len): a launch over a uniform partition passes it for seg_size */
+inline uint32_t crc_init_term(const CrcConsts &c, uint64_t len) { return gf2_mulmod(0xffffffffu, gf2_xpow(c.x2n, 8ull * len)); }
+
+/* one row step of a state: byte k of s picks entry k of this lane's copy of table k. The byte comes out of a PRMT and the
+ * address of an IMAD by k128 = 128 (the stride between entries), which the compiler cannot turn into shifts and LEAs, so the
+ * address arithmetic runs on the FMA pipe and the integer-ALU pipe is left with the byte extraction and the xors. */
+#define MZ_CRC_STEP(s, w)                                                                                                    \
+    (s) = sm.ld32_a(MZ_BYTE(s, 0) * k128 + a0) ^ sm.ld32_a(MZ_BYTE(s, 1) * k128 + a1) ^ sm.ld32_a(MZ_BYTE(s, 2) * k128 + a2) ^ \
+          sm.ld32_a(MZ_BYTE(s, 3) * k128 + a3) ^ (w)
 
 /* gather up to 16 bytes of a right-aligned virtual row: virtual byte index vb = lane*16 + i maps to
  * data[vb - (512 - n)] when that is >= 0 */
 __device__ __forceinline__ uint4 crc_virtual_row(const uint8_t *data, uint32_t n, unsigned lane) {
     uint32_t w[4] = {0, 0, 0, 0};
     int shift = (int)CRC_ROW - (int)n;
+#pragma unroll
     for (int i = 0; i < 16; i++) {
         int vb = (int)lane * 16 + i;
         if (vb >= shift) w[i >> 2] |= (uint32_t)data[vb - shift] << (8 * (i & 3));
@@ -93,11 +109,12 @@ __device__ __forceinline__ uint4 crc_virtual_row(const uint8_t *data, uint32_t n
     return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
+/* sum over the lane's slots j of s_j x^(32 (128 - 4 lane - j)): Horner over the four slots by x^32, then one multiplication by
+ * the last slot's x^(32 (125 - 4 lane)) */
 __device__ __forceinline__ uint32_t crc_warp_finalize(uint32_t s0, uint32_t s1, uint32_t s2, uint32_t s3, const CrcConsts *cc,
                                                       unsigned lane) {
-    uint32_t r = gf2_mulmod(s0, cc->slot_mul[4 * lane + 0]) ^ gf2_mulmod(s1, cc->slot_mul[4 * lane + 1]) ^
-                 gf2_mulmod(s2, cc->slot_mul[4 * lane + 2]) ^ gf2_mulmod(s3, cc->slot_mul[4 * lane + 3]);
-    return __reduce_xor_sync(MZ_FULL_MASK, r);
+    const uint32_t u = gf2_mul_x32(gf2_mul_x32(gf2_mul_x32(s0) ^ s1) ^ s2) ^ s3;
+    return __reduce_xor_sync(MZ_FULL_MASK, gf2_mulmod(u, cc->slot_mul[4 * lane + 3]));
 }
 
 __global__ void __launch_bounds__(CRC_THREADS, 1) crc32_segments_kernel(CrcParams P) {
@@ -107,7 +124,10 @@ __global__ void __launch_bounds__(CRC_THREADS, 1) crc32_segments_kernel(CrcParam
     /* replicate the 4 KiB of tables 32 times, one copy per bank */
     for (uint32_t i = threadIdx.x; i < CRC_TABLE_WORDS; i += CRC_THREADS) tab[i] = (&P.consts->row_tab[0][0])[i >> 5];
     __syncthreads();
-    const uint32_t *t0 = tab + lane, *t1 = t0 + 256 * 32, *t2 = t1 + 256 * 32, *t3 = t2 + 256 * 32;
+    Smem sm;
+    sm.init(smem);
+    const uint32_t a0 = sm.addr(lane * 4), a1 = a0 + 256 * 32 * 4, a2 = a1 + 256 * 32 * 4, a3 = a2 + 256 * 32 * 4;
+    const uint32_t k128 = blockDim.x / (CRC_THREADS / 128); /* 128, opaque to the compiler */
 
     const uint32_t nwarps = gridDim.x * (CRC_THREADS / 32);
     for (uint32_t seg = blockIdx.x * (CRC_THREADS / 32) + warp_id(); seg < P.nseg; seg += nwarps) {
@@ -133,17 +153,28 @@ __global__ void __launch_bounds__(CRC_THREADS, 1) crc32_segments_kernel(CrcParam
         uint64_t rows = (len - head) / CRC_ROW;
         const uint4 *rp = (const uint4 *)q + lane;
         uint64_t r = 0;
-        for (; r + CRC_UNROLL <= rows; r += CRC_UNROLL) {
+        if (rows >= CRC_UNROLL) {
+            /* software pipeline: batch r + CRC_UNROLL is loaded before batch r is folded, so a warp always has rows in flight */
             uint4 w[CRC_UNROLL];
 #pragma unroll
-            for (int u = 0; u < CRC_UNROLL; u++) w[u] = ldg_stream(rp + (r + u) * (CRC_ROW / 16));
+            for (int u = 0; u < CRC_UNROLL; u++) w[u] = ldg_stream(rp + (uint64_t)u * (CRC_ROW / 16));
+            for (;; r += CRC_UNROLL) {
+                const bool more = r + 2 * CRC_UNROLL <= rows;
+                uint4 nx[CRC_UNROLL];
 #pragma unroll
-            for (int u = 0; u < CRC_UNROLL; u++) {
-                MZ_CRC_STEP(s0, w[u].x);
-                MZ_CRC_STEP(s1, w[u].y);
-                MZ_CRC_STEP(s2, w[u].z);
-                MZ_CRC_STEP(s3, w[u].w);
+                for (int u = 0; u < CRC_UNROLL; u++) nx[u] = more ? ldg_stream(rp + (r + CRC_UNROLL + u) * (CRC_ROW / 16)) : w[u];
+#pragma unroll
+                for (int u = 0; u < CRC_UNROLL; u++) {
+                    MZ_CRC_STEP(s0, w[u].x);
+                    MZ_CRC_STEP(s1, w[u].y);
+                    MZ_CRC_STEP(s2, w[u].z);
+                    MZ_CRC_STEP(s3, w[u].w);
+                }
+                if (!more) break;
+#pragma unroll
+                for (int u = 0; u < CRC_UNROLL; u++) w[u] = nx[u];
             }
+            r += CRC_UNROLL;
         }
         for (; r < rows; r++) {
             uint4 w = ldg_stream(rp + r * (CRC_ROW / 16));
@@ -162,7 +193,10 @@ __global__ void __launch_bounds__(CRC_THREADS, 1) crc32_segments_kernel(CrcParam
         }
         if (lane == 0) {
             P.out_residue[seg] = res;
-            if (P.out_crc) P.out_crc[seg] = ~(gf2_mulmod(0xffffffffu, gf2_xpow(cc->x2n, 8ull * len)) ^ res);
+            if (P.out_crc) {
+                const uint32_t init = P.init_len && len == P.init_len ? P.init : gf2_mulmod(0xffffffffu, gf2_xpow(cc->x2n, 8ull * len));
+                P.out_crc[seg] = ~(init ^ res);
+            }
         }
     }
 }

@@ -117,6 +117,12 @@ uint64_t pick_crc_seg(uint64_t len, int sm_count) {
     return seg;
 }
 
+/* the join's persistent grid: as many CTAs as are resident, and no more than one warp per slot */
+uint32_t gather_grid(uint32_t nchunks, int sm_count) {
+    const uint32_t need = (nchunks + GATHER_THREADS / 32 - 1) / (GATHER_THREADS / 32), resident = (uint32_t)sm_count * GATHER_CTAS_PER_SM;
+    return need < resident ? need : resident;
+}
+
 } // namespace
 
 extern "C" {
@@ -259,6 +265,8 @@ int32_t mz_cuda_crc32_segments(const void *d_in, uint64_t total_len, uint64_t se
     P.consts = c->d_consts;
     P.out_residue = d_residue;
     P.out_crc = d_crc;
+    P.init_len = d_off ? 0 : seg_size; /* every segment but perhaps the last has seg_size bytes */
+    P.init = d_off ? 0u : crc_init_term(g_consts, seg_size);
     uint32_t warps_per_cta = CRC_THREADS / 32;
     uint32_t grid = (nseg + warps_per_cta - 1) / warps_per_cta;
     if (grid > (uint32_t)c->sm_count) grid = (uint32_t)c->sm_count;
@@ -406,11 +414,8 @@ int32_t mz_cuda_concat(const void *d_slots, uint64_t slot_stride, const uint32_t
     int32_t err = get_ctx(&c);
     if (err) return err;
     MZ_LAUNCH(scan_lengths_kernel, dim3(1), dim3(SCAN_THREADS), 0, (cudaStream_t)stream, d_out_len, nchunks, (uint64_t)0, d_offsets);
-    if (nchunks) {
-        uint32_t grid = nchunks < (uint32_t)c->sm_count * 16u ? nchunks : (uint32_t)c->sm_count * 16u;
-        MZ_LAUNCH(gather_slots_kernel, dim3(grid), dim3(GATHER_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_slots, slot_stride,
-                  d_out_len, (const uint64_t *)d_offsets, nchunks, (uint8_t *)d_dst);
-    }
+    if (nchunks) MZ_LAUNCH(gather_slots_kernel, dim3(gather_grid(nchunks, c->sm_count)), dim3(GATHER_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_slots,
+                           slot_stride, d_out_len, (const uint64_t *)d_offsets, nchunks, (uint8_t *)d_dst);
     CK(cudaGetLastError());
     return MZ_OK;
 }
@@ -421,9 +426,8 @@ int32_t mz_cuda_gather(const void *d_slots, uint64_t slot_stride, const uint32_t
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (nchunks == 0) return MZ_OK;
-    uint32_t grid = nchunks < (uint32_t)c->sm_count * 16u ? nchunks : (uint32_t)c->sm_count * 16u;
-    MZ_LAUNCH(gather_slots_kernel, dim3(grid), dim3(GATHER_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_slots, slot_stride, d_out_len, d_offsets,
-              nchunks, (uint8_t *)d_dst);
+    MZ_LAUNCH(gather_slots_kernel, dim3(gather_grid(nchunks, c->sm_count)), dim3(GATHER_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_slots, slot_stride,
+              d_out_len, d_offsets, nchunks, (uint8_t *)d_dst);
     CK(cudaGetLastError());
     return MZ_OK;
 }
