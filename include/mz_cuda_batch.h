@@ -171,6 +171,49 @@ typedef struct mz_cuda_inflate_state {
 int32_t mz_cuda_inflate_streams(const mz_cuda_inflate_job *d_jobs, mz_cuda_inflate_state *d_states, uint32_t nstreams,
                                 void *stream);
 
+/* ---- K9: zip entries located, copied and verified on the device (csrc/zipdir_kernel.cuh) ------------------------------
+ * A round = the stored bytes of n zip entries in one device buffer + one record per entry from the central directory. */
+typedef struct mz_cuda_zip_ent {
+    uint64_t src_off;   /* in the round's buffer: the entry's local header, or (MZ_CUDA_ZIP_ENT_AT_DATA) its stored bytes */
+    uint64_t src_len;   /* the entry's extent: nothing of it lies past src_off + src_len */
+    uint64_t csize;     /* stored bytes as recorded (WinZip AES: salt + verifier + ciphertext + authentication code) */
+    uint64_t usize;     /* plain bytes as recorded */
+    uint64_t out_off;   /* the plain bytes go to out + out_off (16-byte aligned) */
+    uint32_t crc;       /* CRC-32 as recorded */
+    uint32_t job;       /* DEFLATE entries: index of the entry's K5 job and state */
+    uint32_t aes_slot;  /* WinZip AES entries: row of the K8 tables (salt, keys, MAC, ciphertext offset / length) */
+    uint32_t sha_slot;  /* row of the expected SHA-256 digests, or 0xffffffff */
+    uint16_t method;    /* 0 (STORE) or 8 (DEFLATE) */
+    uint8_t aes;        /* 0, or the WinZip AES strength 1..3 */
+    uint8_t flags;      /* MZ_CUDA_ZIP_ENT_AT_DATA */
+    uint32_t pad;
+} mz_cuda_zip_ent;
+#define MZ_CUDA_ZIP_ENT_AT_DATA 1u
+
+typedef struct mz_cuda_zip_round { /* device pointers; per entry unless noted */
+    const void *buf;               /* the round's stored bytes, 32 readable bytes past buf_len */
+    uint64_t buf_len;
+    void *out;                     /* plain bytes */
+    const mz_cuda_zip_ent *ent;
+    uint32_t n, pad;
+    mz_cuda_inflate_job *jobs;     /* per DEFLATE entry (written by locate) */
+    const mz_cuda_inflate_state *states;
+    uint64_t *seg_off, *seg_len64, *data_off; /* written by locate: the plain bytes' segment (K1 / K7), the stream's start in buf */
+    uint32_t *seg_len;
+    const uint32_t *crc;           /* K1 result over seg_* */
+    const void *digest;            /* K7 result over seg_*, 32 bytes per entry (read only for entries with a sha_slot) */
+    const void *sha_expect;        /* 32 bytes per sha_slot */
+    void *salt;                    /* per aes_slot: 16 bytes (written by locate) */
+    uint64_t *coff, *clen;         /* per aes_slot: ciphertext offset in buf and length (written by locate) */
+    const void *keys, *mac;        /* per aes_slot: K8 key records and HMACs */
+    uint32_t *status;              /* 0, or class << 24 | -MZ_code (1 locate, 2 AES, 3 stream / CRC / hash) */
+} mz_cuda_zip_round;
+/* locate: status, jobs, seg_*, data_off, salt / coff / clen. stored: STORE entries' bytes to out. verify: the final status words
+ * (needs keys / mac for AES entries, states, crc, digest). */
+int32_t mz_cuda_zip_locate(const mz_cuda_zip_round *round, void *stream);
+int32_t mz_cuda_zip_copy_stored(const mz_cuda_zip_round *round, void *stream);
+int32_t mz_cuda_zip_verify(const mz_cuda_zip_round *round, void *stream);
+
 /* ---- K6: one long foreign stream, segment-speculative (csrc/inflate_spec_kernel.cuh) ------------------------
  * One ROUND decodes as much of the compressed window d_in[0..in_avail) as can be proven, starting at the block
  * boundary `start_bit` (absolute bit; the serial decoder's state must be at a block header), into

@@ -107,6 +107,29 @@ int32_t mz_zip_cuda_extract_all(void *zip_handle, mz_cuda_zip_entry_cb cb, void 
  * return MZ_SUPPORT_ERROR; encrypted entries without a password MZ_PASSWORD_ERROR. */
 int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_cuda_zip_entry_cb cb, void *userdata, mz_cuda_zip_stats *stats);
 
+/* ---- a whole archive, natively (scope row f2) ---------------------------------------------------------------------------
+ * Extracts every entry of the archive readable from base_stream (any mz_stream: file, buffered, memory, mem64). The call needs no
+ * mz_zip handle and no zip container in the process: it reads the end records (incl. zip64) and the whole central directory
+ * itself, corrects for prepended data as the reference does (self-extracting archives), and reads each round's stored bytes with
+ * one base read per run of adjacent entries. The device checks every local header (K9), decrypts (K8), inflates (K5), copies
+ * STORE entries, and verifies CRC-32, SHA-256 (MZ_ZIP_EXTENSION_HASH) and the AES verifier and HMAC. Up to four rounds are in
+ * flight, each on its own thread and CUDA stream; MZ_ZIP_CUDA_ALL_DEVICES sends them round-robin to every visible GPU.
+ * `cb` as for mz_zip_cuda_extract_all: once per entry in central-directory order, on the caller's thread; a round is delivered
+ * only when all its entries verified. Entries handled and errors: those of mz_zip_cuda_extract_all_aes (password may be NULL when
+ * no entry is encrypted); MZ_FORMAT_ERROR for a missing or inconsistent end record, directory or local header; MZ_SUPPORT_ERROR
+ * also for split archives. Errors of the archive as a whole (end records, directory location) are returned before anything is
+ * delivered. Otherwise the first failing entry in directory order decides, as in the reference's reader: an entry the call refuses
+ * (unsupported, no password, malformed record) ends the list, the entries in front of it are delivered, then its error is
+ * returned; a decoding, CRC, hash, AES or local-header error in a round returns that round's first failing entry, and nothing of
+ * that round is delivered; a base read error returns after the rounds read before it. Staging is pooled with the writer's
+ * (MZ_CUDA_ZIP_POOL, mz_zip_cuda_trim); MZ_CUDA_ZIP_ROUND_MB sets the stored bytes per round (default 32; plain bytes up to four
+ * times that). An entry larger than a round gets a round of its own size; the call then keeps one round slot per device instead of
+ * four and does not pool it (an entry of 1 GiB needs about 1 GiB of page-locked input and output staging).
+ * stats: pack_ms = directory parse and base reads (caller's thread), gpu_ms = upload to download summed over rounds,
+ * container_ms = time in the callback, setup_ms = staging set-up and release; bytes_in / bytes_out = stored / plain bytes. */
+int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uint32_t flags, mz_cuda_zip_entry_cb cb, void *userdata,
+                                    mz_cuda_zip_stats *stats);
+
 /* sizeof the mz_zip_file mirror this library was built with: the host asserts it equals sizeof(mz_zip_file) */
 uint32_t mz_zip_cuda_abi_file_info_size(void);
 

@@ -58,8 +58,26 @@ EXPORTS = [
     "mz_cuda_stream_wait_event", "mz_cuda_gather", "mz_cuda_scatter_blobs",
     # include/mz_zip_cuda.h
     "mz_zip_cuda_add_buffers", "mz_zip_cuda_add_buffers_ex", "mz_zip_cuda_write_archive", "mz_zip_cuda_trim", "mz_zip_cuda_write_archive_aes", "mz_zip_cuda_extract_all",
-    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_abi_file_info_size",
+    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_abi_file_info_size",
+    # include/mz_cuda_batch.h, K9
+    "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify",
 ]
+
+# mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
+ZIP_ENTRY_CB = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_uint32)
+MZ_ZIP_CUDA_HASH_SHA256, MZ_ZIP_CUDA_ALL_DEVICES, MZ_ZIP_CUDA_AES = 1, 2, 4
+
+
+class ZipStats(C.Structure):
+    """mz_cuda_zip_stats (include/mz_zip_cuda.h)"""
+    _fields_ = [("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64), ("entries", C.c_uint32), ("rounds", C.c_uint32),
+                ("pack_ms", C.c_double), ("gpu_ms", C.c_double), ("container_ms", C.c_double), ("setup_ms", C.c_double)]
+
+
+class ZipItem(C.Structure):
+    """mz_cuda_zip_item (include/mz_zip_cuda.h)"""
+    _fields_ = [("filename", C.c_char_p), ("data", C.c_void_p), ("size", C.c_int64), ("modified_date", C.c_int64),
+                ("external_fa", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 def load():
@@ -141,6 +159,13 @@ def configure(L):
     sig("mz_cuda_stream_wait_event", i32, [vp, vp])
     sig("mz_cuda_gather", i32, [vp, u64, vp, u32, vp, vp, vp])
     sig("mz_cuda_scatter_blobs", i32, [vp, vp, vp, u32, vp, vp])
+    sig("mz_cuda_zip_locate", i32, [vp, vp])
+    sig("mz_cuda_zip_copy_stored", i32, [vp, vp])
+    sig("mz_cuda_zip_verify", i32, [vp, vp])
+    sig("mz_zip_cuda_write_archive", i32, [vp, vp, u32, C.c_int16, u32, vp])
+    sig("mz_zip_cuda_write_archive_aes", i32, [vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp])
+    sig("mz_zip_cuda_extract_archive", i32, [vp, C.c_char_p, u32, ZIP_ENTRY_CB, vp, vp])
+    sig("mz_zip_cuda_trim", None, [])
     return L
 
 

@@ -17,6 +17,7 @@
 #include "inflate_spec_kernel.cuh"
 #include "sha256_kernel.cuh"
 #include "wzaes_kernel.cuh"
+#include "zipdir_kernel.cuh"
 
 #define MZ_OK 0
 #define MZ_MEM_ERROR (-4)
@@ -29,6 +30,8 @@ using namespace mzc;
 static_assert(sizeof(mz_cuda_inflate_job) == sizeof(InflateJob), "job layout");
 static_assert(sizeof(mz_cuda_inflate_state) == sizeof(InflateState), "state layout");
 static_assert(sizeof(mz_cuda_spec_summary) == sizeof(SpecSummary), "summary layout");
+static_assert(sizeof(mz_cuda_zip_ent) == sizeof(ZipEnt) && sizeof(mz_cuda_zip_ent) == 64, "zip entry layout");
+static_assert(sizeof(mz_cuda_zip_round) == sizeof(ZipRound), "zip round layout");
 
 namespace {
 
@@ -461,6 +464,38 @@ int32_t mz_cuda_inflate_streams(const mz_cuda_inflate_job *d_jobs, mz_cuda_infla
     CK(cudaGetLastError());
     return MZ_OK;
 }
+
+/* ---- K9: zip entries ---------------------------------------------------------------------------------------- */
+namespace {
+int32_t zip_launch(const mz_cuda_zip_round *r, void *stream, int which) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!r) return MZ_PARAM_ERROR;
+    if (r->n == 0) return MZ_OK;
+    if (!r->buf || !r->ent || !r->status || !r->data_off) return MZ_PARAM_ERROR;
+    ZipRound R;
+    memcpy(&R, r, sizeof(R));
+    const uint32_t cap = (uint32_t)c->sm_count * 8u;
+    if (which == 0) {
+        if (!r->jobs || !r->seg_off || !r->seg_len || !r->seg_len64 || !r->salt || !r->coff || !r->clen) return MZ_PARAM_ERROR;
+        MZ_LAUNCH(zip_locate_kernel, dim3((r->n + 255) / 256), dim3(256), 0, (cudaStream_t)stream, R);
+    } else if (which == 1) {
+        if (!r->out) return MZ_PARAM_ERROR;
+        const uint32_t g = (r->n + 7) / 8;
+        MZ_LAUNCH(zip_stored_kernel, dim3(g < cap ? g : cap), dim3(256), 0, (cudaStream_t)stream, R);
+    } else {
+        if (!r->states || !r->crc || !r->clen) return MZ_PARAM_ERROR;
+        MZ_LAUNCH(zip_verify_kernel, dim3((r->n + 255) / 256), dim3(256), 0, (cudaStream_t)stream, R);
+    }
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+} // namespace
+
+int32_t mz_cuda_zip_locate(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 0); }
+int32_t mz_cuda_zip_copy_stored(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 1); }
+int32_t mz_cuda_zip_verify(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 2); }
 
 /* workspace carving for K6 (all pieces 256-byte aligned) */
 static inline uint64_t al256(uint64_t v) { return (v + 255) & ~255ull; }

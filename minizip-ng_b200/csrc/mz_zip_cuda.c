@@ -5,6 +5,7 @@
  * (mz_zip.c:2062-2064) and mz_zip_entry_close (mz_zip.c:2116-2160). Here the codec work of MANY entries is one
  * K2+K3 launch + one K1 launch + one K4 launch per round, and the container calls run with raw = 1.
  */
+#define _GNU_SOURCE /* qsort_r */
 #include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -570,8 +571,11 @@ static void za_release(za_slot *z) {
         za_free(z);
 }
 
+static void zr_trim(void);
+
 void mz_zip_cuda_trim(void) {
     const int32_t dev0 = mz_cuda_get_device();
+    zr_trim();
     pthread_mutex_lock(&g_za_mu);
     for (int i = 0; i < g_za_n; i++) {
         mz_cuda_set_device(g_za_pool[i].device);
@@ -1036,8 +1040,247 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
 }
 
 /* ---- batch extraction ------------------------------------------------------------------------------------------ */
+/* One round of extraction on the device (K9 locate, K8, K9 stored copy, K5, K1, K7, K9 verify): the slot's staging, its CUDA
+ * stream, and the round in flight. Both extractors fill h_in and h_ent and call zr_run; mz_zip_cuda_extract_archive keeps up to
+ * four slots in flight on their own threads and pools them between calls (like the native writer's), mz_zip_cuda_extract_all
+ * runs one synchronously. */
+typedef struct zr_slot_s {
+    size_t in_cap, out_cap;
+    uint32_t max_ent;
+    int32_t device;
+    uint8_t *h_in, *d_in, *h_out, *d_out;
+    mz_cuda_zip_ent *h_ent, *d_ent;
+    uint8_t *h_sha, *d_sha;
+    uint32_t *h_status, *d_status;
+    mz_cuda_inflate_job *d_job;
+    mz_cuda_inflate_state *d_state;
+    uint64_t *d_seg_off, *d_seg_len64, *d_data_off, *d_coff, *d_clen;
+    uint32_t *d_seg_len, *d_residue, *d_crc;
+    uint8_t *d_digest, *d_salt, *d_keys, *d_pw, *d_mac;
+    void *stream;
+    /* the round in flight */
+    uint32_t first, last, n, njobs, nsha, na[4];
+    uint64_t max_clen[4];
+    size_t in_used, out_used;
+    const char *password;
+    int32_t err;
+    double gpu_ms;
+    pthread_t th;
+    int running;
+} zr_slot;
+
+static void zr_free(zr_slot *z) {
+    mz_cuda_host_free(z->h_in);
+    mz_cuda_free(z->d_in);
+    mz_cuda_host_free(z->h_out);
+    mz_cuda_free(z->d_out);
+    mz_cuda_host_free(z->h_ent);
+    mz_cuda_free(z->d_ent);
+    mz_cuda_host_free(z->h_sha);
+    mz_cuda_free(z->d_sha);
+    mz_cuda_host_free(z->h_status);
+    mz_cuda_free(z->d_status);
+    mz_cuda_free(z->d_job);
+    mz_cuda_free(z->d_state);
+    mz_cuda_free(z->d_seg_off);
+    mz_cuda_free(z->d_seg_len64);
+    mz_cuda_free(z->d_data_off);
+    mz_cuda_free(z->d_coff);
+    mz_cuda_free(z->d_clen);
+    mz_cuda_free(z->d_seg_len);
+    mz_cuda_free(z->d_residue);
+    mz_cuda_free(z->d_crc);
+    mz_cuda_free(z->d_digest);
+    mz_cuda_free(z->d_salt);
+    mz_cuda_free(z->d_keys);
+    mz_cuda_free(z->d_pw);
+    mz_cuda_free(z->d_mac);
+    if (z->stream)
+        mz_cuda_stream_destroy(z->stream);
+    memset(z, 0, sizeof(*z));
+}
+
+/* in_cap: stored bytes of a round (+ 64 readable bytes past them); out_cap: plain bytes (+ 512); max_ent: entries */
+static int zr_alloc(zr_slot *z, size_t in_cap, size_t out_cap, uint32_t max_ent, int with_stream) {
+    const size_t n = max_ent;
+    memset(z, 0, sizeof(*z));
+    z->in_cap = in_cap;
+    z->out_cap = out_cap;
+    z->max_ent = max_ent;
+    z->h_in = (uint8_t *)mz_cuda_host_alloc(in_cap + 64);
+    z->d_in = (uint8_t *)mz_cuda_malloc(in_cap + 64);
+    z->h_out = (uint8_t *)mz_cuda_host_alloc(out_cap + 512);
+    z->d_out = (uint8_t *)mz_cuda_malloc(out_cap + 512);
+    z->h_ent = (mz_cuda_zip_ent *)mz_cuda_host_alloc(n * sizeof(mz_cuda_zip_ent));
+    z->d_ent = (mz_cuda_zip_ent *)mz_cuda_malloc(n * sizeof(mz_cuda_zip_ent));
+    z->h_sha = (uint8_t *)mz_cuda_host_alloc(n * 32);
+    z->d_sha = (uint8_t *)mz_cuda_malloc(n * 32);
+    z->h_status = (uint32_t *)mz_cuda_host_alloc(n * 4);
+    z->d_status = (uint32_t *)mz_cuda_malloc(n * 4);
+    z->d_job = (mz_cuda_inflate_job *)mz_cuda_malloc(n * sizeof(mz_cuda_inflate_job));
+    z->d_state = (mz_cuda_inflate_state *)mz_cuda_malloc(n * sizeof(mz_cuda_inflate_state));
+    z->d_seg_off = (uint64_t *)mz_cuda_malloc(n * 8);
+    z->d_seg_len64 = (uint64_t *)mz_cuda_malloc(n * 8);
+    z->d_data_off = (uint64_t *)mz_cuda_malloc(n * 8);
+    z->d_coff = (uint64_t *)mz_cuda_malloc(n * 8);
+    z->d_clen = (uint64_t *)mz_cuda_malloc(n * 8);
+    z->d_seg_len = (uint32_t *)mz_cuda_malloc(n * 4);
+    z->d_residue = (uint32_t *)mz_cuda_malloc(n * 4);
+    z->d_crc = (uint32_t *)mz_cuda_malloc(n * 4);
+    z->d_digest = (uint8_t *)mz_cuda_malloc(n * 32);
+    z->d_salt = (uint8_t *)mz_cuda_malloc(n * 16);
+    z->d_keys = (uint8_t *)mz_cuda_malloc(n * MZ_CUDA_WZAES_KEYREC);
+    z->d_pw = (uint8_t *)mz_cuda_malloc(256);
+    z->d_mac = (uint8_t *)mz_cuda_malloc(n * 20);
+    z->stream = with_stream ? mz_cuda_stream_create() : NULL;
+    if (!z->h_in || !z->d_in || !z->h_out || !z->d_out || !z->h_ent || !z->d_ent || !z->h_sha || !z->d_sha || !z->h_status || !z->d_status ||
+        !z->d_job || !z->d_state || !z->d_seg_off || !z->d_seg_len64 || !z->d_data_off || !z->d_coff || !z->d_clen || !z->d_seg_len ||
+        !z->d_residue || !z->d_crc || !z->d_digest || !z->d_salt || !z->d_keys || !z->d_pw || !z->d_mac || (with_stream && !z->stream)) {
+        zr_free(z);
+        return 0;
+    }
+    return 1;
+}
+
+/* the extractor's staging pool: same rules as the writer's (MZ_CUDA_ZIP_POOL=0 off, mz_zip_cuda_trim() empties it) */
+static zr_slot g_zr_pool[ZA_POOL_MAX];
+static int g_zr_n;
+
+static void zr_trim(void) {
+    pthread_mutex_lock(&g_za_mu);
+    for (int i = 0; i < g_zr_n; i++) {
+        mz_cuda_set_device(g_zr_pool[i].device);
+        zr_free(&g_zr_pool[i]);
+    }
+    g_zr_n = 0;
+    pthread_mutex_unlock(&g_za_mu);
+}
+
+static int zr_acquire(zr_slot *z, int32_t dev, size_t in_cap, size_t out_cap, uint32_t max_ent) {
+    int hit = 0;
+    pthread_mutex_lock(&g_za_mu);
+    for (int i = 0; i < g_zr_n; i++) {
+        const zr_slot *q = &g_zr_pool[i];
+        if (q->device == dev && q->in_cap >= in_cap && q->out_cap >= out_cap && q->max_ent >= max_ent) {
+            *z = *q;
+            g_zr_pool[i] = g_zr_pool[--g_zr_n];
+            hit = 1;
+            break;
+        }
+    }
+    pthread_mutex_unlock(&g_za_mu);
+    if (!hit && !zr_alloc(z, in_cap, out_cap, max_ent, 1))
+        return 0;
+    z->device = dev;
+    z->running = 0;
+    z->err = 0;
+    return 1;
+}
+
+static void zr_release(zr_slot *z) {
+    int kept = 0;
+    if (z->h_in && z->stream && za_pool_enabled()) {
+        pthread_mutex_lock(&g_za_mu);
+        if (g_zr_n < ZA_POOL_MAX) {
+            g_zr_pool[g_zr_n++] = *z;
+            kept = 1;
+        }
+        pthread_mutex_unlock(&g_za_mu);
+    }
+    if (kept)
+        memset(z, 0, sizeof(*z));
+    else
+        zr_free(z);
+}
+
+/* the round's device work; on return h_status and h_out hold the results (z->err: a CUDA error, not an entry's) */
+static void *zr_run(void *arg) {
+    zr_slot *z = (zr_slot *)arg;
+    const double t0 = now_ms();
+    void *s = z->stream;
+    const uint32_t n = z->n;
+    int32_t err = mz_cuda_set_device(z->device);
+    mz_cuda_zip_round R;
+    memset(&R, 0, sizeof(R));
+    R.buf = z->d_in;
+    R.buf_len = z->in_used;
+    R.out = z->d_out;
+    R.ent = z->d_ent;
+    R.n = n;
+    R.jobs = z->d_job;
+    R.states = z->d_state;
+    R.seg_off = z->d_seg_off;
+    R.seg_len64 = z->d_seg_len64;
+    R.data_off = z->d_data_off;
+    R.seg_len = z->d_seg_len;
+    R.crc = z->d_crc;
+    R.digest = z->d_digest;
+    R.sha_expect = z->d_sha;
+    R.salt = z->d_salt;
+    R.coff = z->d_coff;
+    R.clen = z->d_clen;
+    R.keys = z->d_keys;
+    R.mac = z->d_mac;
+    R.status = z->d_status;
+    if (!err) err = mz_cuda_memcpy_h2d(z->d_in, z->h_in, z->in_used + 32, s); /* K5 reads up to 16 bytes past a stream */
+    if (!err) err = mz_cuda_memcpy_h2d(z->d_ent, z->h_ent, (size_t)n * sizeof(mz_cuda_zip_ent), s);
+    if (!err && z->nsha) err = mz_cuda_memcpy_h2d(z->d_sha, z->h_sha, (size_t)z->nsha * 32, s);
+    if (!err) err = mz_cuda_zip_locate(&R, s);
+    /* WinZip AES (mz_strm_wzaes.c): keys from password + salt, HMAC of the ciphertext, then the ciphertext becomes the compressed
+     * stream in place; one pass per strength present, rows of a strength are contiguous from base */
+    for (uint32_t st = 1, base = 0; st <= 3 && !err; base += z->na[st], st++) {
+        if (!z->na[st])
+            continue;
+        const size_t pwl = strlen(z->password);
+        err = mz_cuda_memcpy_h2d(z->d_pw, z->password, pwl ? pwl : 1, s);
+        if (!err) err = mz_cuda_wzaes_derive(z->d_pw, (uint32_t)pwl, z->d_salt + (size_t)base * 16, z->na[st], st, z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC, s);
+        if (!err) err = mz_cuda_wzaes_hmac(z->d_in, z->d_coff + base, z->d_clen + base, z->na[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC, st,
+                                           z->d_mac + (size_t)base * 20, s);
+        if (!err) err = mz_cuda_wzaes_ctr(z->d_in, z->d_coff + base, z->d_clen + base, z->na[st], z->max_clen[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC,
+                                          st, s);
+    }
+    if (!err) err = mz_cuda_zip_copy_stored(&R, s);
+    if (!err && z->njobs) {
+        err = mz_cuda_memset(z->d_state, 0, (size_t)z->njobs * sizeof(mz_cuda_inflate_state), s);
+        if (!err) err = mz_cuda_inflate_streams(z->d_job, z->d_state, z->njobs, s);
+    }
+    if (!err) err = mz_cuda_crc32_segments(z->d_out, 0, 0, z->d_seg_off, z->d_seg_len, n, z->d_residue, z->d_crc, s);
+    if (!err && z->nsha) err = mz_cuda_sha256_batch(z->d_out, z->d_seg_off, z->d_seg_len64, n, z->d_digest, s);
+    if (!err) err = mz_cuda_zip_verify(&R, s);
+    if (!err) err = mz_cuda_memcpy_d2h(z->h_status, z->d_status, (size_t)n * 4, s);
+    if (!err) err = mz_cuda_memcpy_d2h(z->h_out, z->d_out, z->out_used, s);
+    if (!err) err = mz_cuda_stream_sync(s);
+    z->err = err;
+    z->gpu_ms = now_ms() - t0;
+    return NULL;
+}
+
+/* the round's verdict from the status words. archive_order (mz_zip_cuda_extract_archive): the first failing entry decides, as in
+ * the reference's reader. Otherwise (mz_zip_cuda_extract_all, unchanged): locate errors first (there are none: its records point at
+ * the data), then WinZip AES errors by strength and entry, then stream / CRC / hash errors by entry. */
+static int32_t zr_verdict(const zr_slot *z, int archive_order) {
+    if (archive_order) {
+        for (uint32_t i = 0; i < z->n; i++)
+            if (z->h_status[i])
+                return -(int32_t)(z->h_status[i] & 0xffffu);
+        return MZ_OK;
+    }
+    for (uint32_t i = 0; i < z->n; i++)
+        if ((z->h_status[i] >> 24) == 1)
+            return -(int32_t)(z->h_status[i] & 0xffffu);
+    for (uint32_t st = 1; st <= 3; st++)
+        for (uint32_t i = 0; i < z->n; i++)
+            if (z->h_ent[i].aes == st && (z->h_status[i] >> 24) == 2)
+                return -(int32_t)(z->h_status[i] & 0xffffu);
+    for (uint32_t i = 0; i < z->n; i++)
+        if (z->h_status[i])
+            return -(int32_t)(z->h_status[i] & 0xffffu);
+    return MZ_OK;
+}
+
+/* host-side description of an entry (both extractors) */
 typedef struct zx_entry_s {
-    uint64_t coff, csize, ooff, usize; /* offsets inside the round's compressed / plain buffers */
+    uint64_t off, csize, usize, ext; /* extract_all: offset in the round's staging; native: absolute offset of the local header, extent */
     uint32_t crc, name_off;
     uint16_t method;
     uint8_t has_sha;
@@ -1045,243 +1288,108 @@ typedef struct zx_entry_s {
     uint8_t sha[32]; /* expected SHA-256 from the MZ_ZIP_EXTENSION_HASH extra field */
 } zx_entry;
 
-typedef struct zx_bufs_s {
-    size_t comp_cap, out_cap;
-    uint32_t max_entries;
-    uint8_t *h_comp, *d_comp, *d_out, *h_out;
-    mz_cuda_inflate_job *h_job, *d_job;
-    mz_cuda_inflate_state *h_state, *d_state;
-    uint64_t *h_off, *d_off;
-    uint32_t *h_len, *d_len, *d_residue, *d_crc, *h_crc;
-    uint64_t *h_len64, *d_len64;
-    uint8_t *d_digest, *h_digest;
-    /* WinZip AES entries of the round, grouped by strength (K8) */
-    uint8_t *h_salt, *d_salt, *h_keys, *d_keys, *d_pw, *h_mac, *d_mac;
-    uint64_t *h_coff, *d_coff, *h_clen, *d_clen;
-    uint32_t *aes_idx;
-    zx_entry *ent;
-    char *names;
-    size_t names_cap;
-} zx_bufs;
-
-static void zx_free(zx_bufs *b) {
-    mz_cuda_host_free(b->h_comp);
-    mz_cuda_free(b->d_comp);
-    mz_cuda_free(b->d_out);
-    mz_cuda_host_free(b->h_out);
-    mz_cuda_host_free(b->h_job);
-    mz_cuda_free(b->d_job);
-    mz_cuda_host_free(b->h_state);
-    mz_cuda_free(b->d_state);
-    mz_cuda_host_free(b->h_off);
-    mz_cuda_free(b->d_off);
-    mz_cuda_host_free(b->h_len);
-    mz_cuda_free(b->d_len);
-    mz_cuda_free(b->d_residue);
-    mz_cuda_free(b->d_crc);
-    mz_cuda_host_free(b->h_crc);
-    mz_cuda_host_free(b->h_len64);
-    mz_cuda_free(b->d_len64);
-    mz_cuda_free(b->d_digest);
-    mz_cuda_host_free(b->h_digest);
-    mz_cuda_host_free(b->h_salt);
-    mz_cuda_free(b->d_salt);
-    mz_cuda_host_free(b->h_keys);
-    mz_cuda_free(b->d_keys);
-    mz_cuda_free(b->d_pw);
-    mz_cuda_host_free(b->h_mac);
-    mz_cuda_free(b->d_mac);
-    mz_cuda_host_free(b->h_coff);
-    mz_cuda_free(b->d_coff);
-    mz_cuda_host_free(b->h_clen);
-    mz_cuda_free(b->d_clen);
-    free(b->aes_idx);
-    free(b->ent);
-    free(b->names);
-    memset(b, 0, sizeof(*b));
+/* the records of entries [first, last) into z->h_ent / h_sha, with src_off[k] for entry first + k; plain bytes packed 16-byte aligned */
+static void zr_table(zr_slot *z, const zx_entry *ent, uint32_t first, uint32_t last, const uint64_t *src_off, uint8_t flags) {
+    const uint32_t n = last - first;
+    uint32_t base[4] = {0, 0, 0, 0};
+    memset(z->na, 0, sizeof(z->na));
+    memset(z->max_clen, 0, sizeof(z->max_clen));
+    for (uint32_t k = 0; k < n; k++)
+        z->na[ent[first + k].aes & 3]++;
+    base[2] = z->na[1];
+    base[3] = z->na[1] + z->na[2];
+    z->na[0] = 0;
+    uint32_t fill[4] = {0, 0, 0, 0};
+    size_t out = 0;
+    z->n = n;
+    z->njobs = z->nsha = 0;
+    for (uint32_t k = 0; k < n; k++) {
+        const zx_entry *e = &ent[first + k];
+        mz_cuda_zip_ent *r = &z->h_ent[k];
+        memset(r, 0, sizeof(*r));
+        r->src_off = src_off[k];
+        r->src_len = (flags & MZ_CUDA_ZIP_ENT_AT_DATA) ? e->csize : e->ext;
+        r->csize = e->csize;
+        r->usize = e->usize;
+        r->out_off = out;
+        r->crc = e->crc;
+        r->method = e->method;
+        r->aes = e->aes;
+        r->flags = flags;
+        r->job = e->method == 8 ? z->njobs++ : 0xffffffffu;
+        r->aes_slot = e->aes ? base[e->aes] + fill[e->aes]++ : 0xffffffffu;
+        if (e->aes) {
+            const uint64_t clen = e->csize - (4u * e->aes + 4u + 12u);
+            if (clen > z->max_clen[e->aes]) z->max_clen[e->aes] = clen;
+        }
+        r->sha_slot = 0xffffffffu;
+        if (e->has_sha) {
+            memcpy(z->h_sha + (size_t)z->nsha * 32, e->sha, 32);
+            r->sha_slot = z->nsha++;
+        }
+        out += ((size_t)e->usize + 15) & ~(size_t)15;
+    }
+    z->out_used = out;
 }
 
-/* the K8 tables, made when the first encrypted entry turns up */
-static int zx_alloc_aes(zx_bufs *b) {
-    const size_t n = b->max_entries;
-    if (b->aes_idx)
-        return 1;
-    b->h_salt = (uint8_t *)mz_cuda_host_alloc(n * 16);
-    b->d_salt = (uint8_t *)mz_cuda_malloc(n * 16);
-    b->h_keys = (uint8_t *)mz_cuda_host_alloc(n * MZ_CUDA_WZAES_KEYREC);
-    b->d_keys = (uint8_t *)mz_cuda_malloc(n * MZ_CUDA_WZAES_KEYREC);
-    b->d_pw = (uint8_t *)mz_cuda_malloc(256);
-    b->h_mac = (uint8_t *)mz_cuda_host_alloc(n * 20);
-    b->d_mac = (uint8_t *)mz_cuda_malloc(n * 20);
-    b->h_coff = (uint64_t *)mz_cuda_host_alloc(n * 8);
-    b->d_coff = (uint64_t *)mz_cuda_malloc(n * 8);
-    b->h_clen = (uint64_t *)mz_cuda_host_alloc(n * 8);
-    b->d_clen = (uint64_t *)mz_cuda_malloc(n * 8);
-    b->aes_idx = (uint32_t *)malloc(n * 4);
-    return b->h_salt && b->d_salt && b->h_keys && b->d_keys && b->d_pw && b->h_mac && b->d_mac && b->h_coff && b->d_coff && b->h_clen && b->d_clen &&
-           b->aes_idx;
-}
-
-static int zx_alloc(zx_bufs *b, size_t comp_cap, size_t out_cap, uint32_t max_entries) {
-    memset(b, 0, sizeof(*b));
-    b->comp_cap = comp_cap;
-    b->out_cap = out_cap;
-    b->max_entries = max_entries;
-    b->names_cap = (size_t)max_entries * 64;
-    b->h_comp = (uint8_t *)mz_cuda_host_alloc(comp_cap + 64);
-    b->d_comp = (uint8_t *)mz_cuda_malloc(comp_cap + 64);
-    b->d_out = (uint8_t *)mz_cuda_malloc(out_cap + 512);
-    b->h_out = (uint8_t *)mz_cuda_host_alloc(out_cap + 512);
-    b->h_job = (mz_cuda_inflate_job *)mz_cuda_host_alloc((size_t)max_entries * sizeof(mz_cuda_inflate_job));
-    b->d_job = (mz_cuda_inflate_job *)mz_cuda_malloc((size_t)max_entries * sizeof(mz_cuda_inflate_job));
-    b->h_state = (mz_cuda_inflate_state *)mz_cuda_host_alloc((size_t)max_entries * sizeof(mz_cuda_inflate_state));
-    b->d_state = (mz_cuda_inflate_state *)mz_cuda_malloc((size_t)max_entries * sizeof(mz_cuda_inflate_state));
-    b->h_off = (uint64_t *)mz_cuda_host_alloc((size_t)max_entries * 8);
-    b->d_off = (uint64_t *)mz_cuda_malloc((size_t)max_entries * 8);
-    b->h_len = (uint32_t *)mz_cuda_host_alloc((size_t)max_entries * 4);
-    b->d_len = (uint32_t *)mz_cuda_malloc((size_t)max_entries * 4);
-    b->d_residue = (uint32_t *)mz_cuda_malloc((size_t)max_entries * 4);
-    b->d_crc = (uint32_t *)mz_cuda_malloc((size_t)max_entries * 4);
-    b->h_crc = (uint32_t *)mz_cuda_host_alloc((size_t)max_entries * 4);
-    b->h_len64 = (uint64_t *)mz_cuda_host_alloc((size_t)max_entries * 8);
-    b->d_len64 = (uint64_t *)mz_cuda_malloc((size_t)max_entries * 8);
-    b->d_digest = (uint8_t *)mz_cuda_malloc((size_t)max_entries * 32);
-    b->h_digest = (uint8_t *)mz_cuda_host_alloc((size_t)max_entries * 32);
-    b->ent = (zx_entry *)malloc((size_t)max_entries * sizeof(zx_entry));
-    b->names = (char *)malloc(b->names_cap);
-    if (!b->h_comp || !b->d_comp || !b->d_out || !b->h_out || !b->h_job || !b->d_job || !b->h_state || !b->d_state || !b->h_off || !b->d_off ||
-        !b->h_len || !b->d_len || !b->d_residue || !b->d_crc || !b->h_crc || !b->h_len64 || !b->d_len64 || !b->d_digest || !b->h_digest ||
-        !b->ent || !b->names) {
-        zx_free(b);
-        return 0;
-    }
-    return 1;
-}
-
-/* decode + checksum + deliver the entries collected in b->ent[0..n) */
-static int32_t zx_flush(zx_bufs *b, uint32_t n, size_t comp_used, size_t out_used, const char *password, mz_cuda_zip_entry_cb cb, void *userdata,
-                        mz_cuda_zip_stats *st) {
-    int32_t err = MZ_OK;
-    uint32_t njobs = 0;
-    double t0 = now_ms();
-    if (n == 0)
-        return MZ_OK;
-    err = mz_cuda_memcpy_h2d(b->d_comp, b->h_comp, comp_used + 32, NULL);
-    /* WinZip AES entries first (mz_strm_wzaes.c): keys from password + salt, verifier, HMAC of the ciphertext against the stored
-     * authentication code, then the ciphertext becomes the compressed stream in place. One pass per strength present. */
-    for (uint32_t strength = 1; strength <= 3 && !err; strength++) {
-        const uint32_t slen = 4 * strength + 4;
-        uint32_t m = 0;
-        uint64_t max_clen = 0;
-        for (uint32_t i = 0; i < n; i++) {
-            zx_entry *e = &b->ent[i];
-            if (e->aes != strength)
-                continue;
-            memcpy(b->h_salt + (size_t)m * 16, b->h_comp + e->coff, slen);
-            b->h_coff[m] = e->coff + slen + 2;
-            b->h_clen[m] = e->csize - slen - 12;
-            if (b->h_clen[m] > max_clen) max_clen = b->h_clen[m];
-            b->aes_idx[m++] = i;
-        }
-        if (m == 0)
-            continue;
-        const size_t pwl = strlen(password);
-        err = mz_cuda_memcpy_h2d(b->d_salt, b->h_salt, (size_t)m * 16, NULL);
-        if (!err) err = mz_cuda_memcpy_h2d(b->d_pw, password, pwl ? pwl : 1, NULL);
-        if (!err) err = mz_cuda_wzaes_derive(b->d_pw, (uint32_t)pwl, b->d_salt, m, strength, b->d_keys, NULL);
-        if (!err) err = mz_cuda_memcpy_d2h(b->h_keys, b->d_keys, (size_t)m * MZ_CUDA_WZAES_KEYREC, NULL);
-        if (!err) err = mz_cuda_memcpy_h2d(b->d_coff, b->h_coff, (size_t)m * 8, NULL);
-        if (!err) err = mz_cuda_memcpy_h2d(b->d_clen, b->h_clen, (size_t)m * 8, NULL);
-        if (!err) err = mz_cuda_wzaes_hmac(b->d_comp, b->d_coff, b->d_clen, m, b->d_keys, strength, b->d_mac, NULL);
-        if (!err) err = mz_cuda_memcpy_d2h(b->h_mac, b->d_mac, (size_t)m * 20, NULL);
-        if (!err) err = mz_cuda_wzaes_ctr(b->d_comp, b->d_coff, b->d_clen, m, max_clen, b->d_keys, strength, NULL);
-        if (!err) err = mz_cuda_stream_sync(NULL);
-        for (uint32_t k = 0; k < m && !err; k++) {
-            zx_entry *e = &b->ent[b->aes_idx[k]];
-            if (memcmp(b->h_keys + (size_t)k * MZ_CUDA_WZAES_KEYREC + 64, b->h_comp + e->coff + slen, 2) != 0)
-                err = MZ_PASSWORD_ERROR; /* mz_strm_wzaes.c:133-134 */
-            else if (memcmp(b->h_mac + (size_t)k * 20, b->h_comp + b->h_coff[k] + b->h_clen[k], 10) != 0)
-                err = MZ_CRC_ERROR;      /* :252-254 */
-            e->coff = b->h_coff[k];      /* from here on the entry is its compressed stream */
-            e->csize = b->h_clen[k];
-        }
-    }
-    if (err)
-        return err;
-    memset(b->h_state, 0, (size_t)n * sizeof(mz_cuda_inflate_state));
-    for (uint32_t i = 0; i < n; i++) {
-        const zx_entry *e = &b->ent[i];
-        b->h_off[i] = e->ooff;
-        b->h_len[i] = (uint32_t)e->usize;
-        if (e->method == 8) {
-            mz_cuda_inflate_job *j = &b->h_job[njobs];
-            j->d_in = b->d_comp + e->coff;
-            j->in_base = 0;
-            j->in_avail = e->csize;
-            j->d_out = b->d_out + e->ooff;
-            j->out_base = 0;
-            j->out_cap = e->usize;
-            j->in_final = 1;
-            j->flags = 0;
-            njobs++;
-        }
-    }
-    /* stored entries: their bytes are the plain bytes */
-    for (uint32_t i = 0; i < n && !err; i++)
-        if (b->ent[i].method == 0 && b->ent[i].usize)
-            err = mz_cuda_memcpy_d2d(b->d_out + b->ent[i].ooff, b->d_comp + b->ent[i].coff, (size_t)b->ent[i].usize, NULL);
-    if (!err && njobs) {
-        err = mz_cuda_memcpy_h2d(b->d_job, b->h_job, (size_t)njobs * sizeof(mz_cuda_inflate_job), NULL);
-        if (!err) err = mz_cuda_memcpy_h2d(b->d_state, b->h_state, (size_t)njobs * sizeof(mz_cuda_inflate_state), NULL);
-        if (!err) err = mz_cuda_inflate_streams(b->d_job, b->d_state, njobs, NULL);
-        if (!err) err = mz_cuda_memcpy_d2h(b->h_state, b->d_state, (size_t)njobs * sizeof(mz_cuda_inflate_state), NULL);
-    }
-    if (!err) err = mz_cuda_memcpy_h2d(b->d_off, b->h_off, (size_t)n * 8, NULL);
-    if (!err) err = mz_cuda_memcpy_h2d(b->d_len, b->h_len, (size_t)n * 4, NULL);
-    if (!err) err = mz_cuda_crc32_segments(b->d_out, 0, 0, b->d_off, b->d_len, n, b->d_residue, b->d_crc, NULL);
-    if (!err) err = mz_cuda_memcpy_d2h(b->h_crc, b->d_crc, (size_t)n * 4, NULL);
-    int any_sha = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        any_sha |= b->ent[i].has_sha;
-        b->h_len64[i] = b->ent[i].usize;
-    }
-    if (!err && any_sha) { /* K7 over the round's plain bytes */
-        err = mz_cuda_memcpy_h2d(b->d_len64, b->h_len64, (size_t)n * 8, NULL);
-        if (!err) err = mz_cuda_sha256_batch(b->d_out, b->d_off, b->d_len64, n, b->d_digest, NULL);
-        if (!err) err = mz_cuda_memcpy_d2h(b->h_digest, b->d_digest, (size_t)n * 32, NULL);
-    }
-    if (!err) err = mz_cuda_memcpy_d2h(b->h_out, b->d_out, out_used, NULL);
-    if (!err) err = mz_cuda_stream_sync(NULL);
-    double t1 = now_ms();
-    if (err)
-        return err;
-    uint32_t jk = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        const zx_entry *e = &b->ent[i];
-        if (e->method == 8) {
-            const mz_cuda_inflate_state *s = &b->h_state[jk++];
-            /* the stream must end, produce exactly the recorded size and use exactly the recorded bytes (mz_zip.c:2116-2128 checks
-             * the same three things through total_in / total_out / crc) */
-            if (s->status != 1 || s->out_pos != e->usize || ((s->in_bitpos + 7) >> 3) != e->csize)
-                return s->status < 0 ? s->status : MZ_DATA_ERROR;
-        }
-        const uint32_t crc = e->usize ? b->h_crc[i] : 0u;
-        if (crc != e->crc)
-            return MZ_CRC_ERROR;
-        if (e->has_sha && memcmp(b->h_digest + (size_t)i * 32, e->sha, 32) != 0)
-            return MZ_CRC_ERROR; /* mz_zip_reader_entry_close: hash mismatch -> MZ_CRC_ERROR (mz_zip_rw.c:444-447) */
-    }
-    double t2 = now_ms();
-    for (uint32_t i = 0; i < n; i++) {
-        const zx_entry *e = &b->ent[i];
+/* hands a verified round to the callback */
+static int32_t zr_deliver(const zr_slot *z, const zx_entry *ent, const char *names, mz_cuda_zip_entry_cb cb, void *userdata, mz_cuda_zip_stats *st) {
+    for (uint32_t k = 0; k < z->n; k++) {
+        const zx_entry *e = &ent[z->first + k];
         if (cb) {
-            err = cb(userdata, b->names + e->name_off, b->h_out + e->ooff, (int64_t)e->usize, e->crc);
+            const int32_t err = cb(userdata, names + e->name_off, z->h_out + z->h_ent[k].out_off, (int64_t)e->usize, e->crc);
             if (err)
                 return err;
         }
         st->bytes_in += e->csize;
         st->bytes_out += e->usize;
     }
+    return MZ_OK;
+}
+
+/* the hash extra field: {id u16, size u16, data}; MZ_ZIP_EXTENSION_HASH with algorithm SHA-256 (mz_zip_rw.c:478-510) */
+static void zx_find_sha(zx_entry *e, const uint8_t *xf, uint32_t xlen) {
+    e->has_sha = 0;
+    for (uint32_t xo = 0; xf && xo + 4 <= xlen;) {
+        const uint8_t *x = xf + xo;
+        const uint32_t id = x[0] | (x[1] << 8), xs = x[2] | (x[3] << 8);
+        if (xo + 4 + xs > xlen)
+            break;
+        if (id == 0x1a51 && xs >= 4 + 32 && (x[4] | (x[5] << 8)) == 23 && (x[6] | (x[7] << 8)) == 32) {
+            memcpy(e->sha, x + 8, 32);
+            e->has_sha = 1;
+            break;
+        }
+        xo += 4 + xs;
+    }
+}
+
+/* decode + checksum + deliver the entries collected in ent[0..n) (extract_all: one round at a time, synchronously) */
+static int32_t zx_flush(zr_slot *z, const zx_entry *ent, uint32_t n, size_t comp_used, const char *names, const char *password, mz_cuda_zip_entry_cb cb,
+                        void *userdata, mz_cuda_zip_stats *st) {
+    if (n == 0)
+        return MZ_OK;
+    uint64_t *src = (uint64_t *)malloc((size_t)n * 8);
+    if (!src)
+        return MZ_MEM_ERROR;
+    for (uint32_t i = 0; i < n; i++)
+        src[i] = ent[i].off;
+    const double t0 = now_ms();
+    zr_table(z, ent, 0, n, src, MZ_CUDA_ZIP_ENT_AT_DATA);
+    free(src);
+    z->first = 0;
+    z->last = n;
+    z->in_used = comp_used;
+    z->password = password;
+    zr_run(z);
+    const double t1 = now_ms();
+    int32_t err = z->err ? z->err : zr_verdict(z, 0);
+    if (err)
+        return err;
+    const double t2 = now_ms();
+    err = zr_deliver(z, ent, names, cb, userdata, st);
+    if (err)
+        return err;
     st->gpu_ms += t1 - t0;
     st->container_ms += now_ms() - t2;
     st->entries += n;
@@ -1294,7 +1402,7 @@ int32_t mz_zip_cuda_extract_all(void *zip_handle, mz_cuda_zip_entry_cb cb, void 
 }
 
 int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_cuda_zip_entry_cb cb, void *userdata, mz_cuda_zip_stats *stats) {
-    zx_bufs b;
+    zr_slot z;
     mz_cuda_zip_stats st;
     int32_t err;
     memset(&st, 0, sizeof(st));
@@ -1316,8 +1424,15 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
         }
     }
     const uint32_t max_entries = 65536;
-    if (!zx_alloc(&b, comp_cap, out_cap, max_entries))
+    const size_t names_cap = (size_t)max_entries * 64;
+    zx_entry *ent = (zx_entry *)malloc((size_t)max_entries * sizeof(zx_entry));
+    char *names = (char *)malloc(names_cap);
+    if (!ent || !names || !zr_alloc(&z, comp_cap, out_cap, max_entries, 0)) {
+        free(ent);
+        free(names);
         return MZ_MEM_ERROR;
+    }
+    z.device = mz_cuda_get_device();
     uint32_t n = 0;
     size_t comp_used = 0, out_used = 0, names_used = 0;
     err = mz_zip_goto_first_entry(zip_handle);
@@ -1340,10 +1455,6 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
             err = MZ_SUPPORT_ERROR; /* PKWARE-encrypted, another codec, or too large for the batch path */
             break;
         }
-        if (enc && !zx_alloc_aes(&b)) {
-            err = MZ_MEM_ERROR;
-            break;
-        }
         if (fi->compression_method == 0 && fi->compressed_size - (int64_t)aes_over != fi->uncompressed_size) {
             err = MZ_FORMAT_ERROR;
             break;
@@ -1351,48 +1462,35 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
         const size_t csz = (size_t)fi->compressed_size, usz = (size_t)fi->uncompressed_size;
         const size_t cneed = (csz + 32 + 15) & ~(size_t)15, oneed = (usz + 15) & ~(size_t)15; /* K5 reads up to 16 bytes past a stream */
         const size_t nlen = strlen(fi->filename) + 1;
-        if (cneed > b.comp_cap || oneed > b.out_cap) { /* one entry larger than a round: not batched */
+        if (cneed > z.in_cap || oneed > z.out_cap) { /* one entry larger than a round: not batched */
             err = MZ_SUPPORT_ERROR;
             break;
         }
-        if (n == b.max_entries || comp_used + cneed > b.comp_cap || out_used + oneed > b.out_cap || names_used + nlen > b.names_cap) {
-            err = zx_flush(&b, n, comp_used, out_used, password, cb, userdata, &st);
+        if (n == z.max_ent || comp_used + cneed > z.in_cap || out_used + oneed > z.out_cap || names_used + nlen > names_cap) {
+            err = zx_flush(&z, ent, n, comp_used, names, password, cb, userdata, &st);
             if (err)
                 break;
             n = 0;
             comp_used = out_used = names_used = 0;
         }
-        zx_entry *e = &b.ent[n];
-        e->coff = comp_used;
+        zx_entry *e = &ent[n];
+        e->off = comp_used;
         e->csize = csz;
-        e->ooff = out_used;
         e->usize = usz;
+        e->ext = csz;
         e->crc = fi->crc;
         e->method = fi->compression_method;
         e->name_off = (uint32_t)names_used;
-        e->has_sha = 0;
         e->aes = enc ? fi->aes_strength : 0;
-        /* extra fields are {id u16, size u16, data}; find MZ_ZIP_EXTENSION_HASH with algorithm SHA-256 (mz_zip_rw.c:478-510) */
-        for (uint32_t xo = 0; fi->extrafield && xo + 4 <= fi->extrafield_size;) {
-            const uint8_t *x = fi->extrafield + xo;
-            const uint32_t id = x[0] | (x[1] << 8), xs = x[2] | (x[3] << 8);
-            if (xo + 4 + xs > fi->extrafield_size)
-                break;
-            if (id == 0x1a51 && xs >= 4 + 32 && (x[4] | (x[5] << 8)) == 23 && (x[6] | (x[7] << 8)) == 32) {
-                memcpy(e->sha, x + 8, 32);
-                e->has_sha = 1;
-                break;
-            }
-            xo += 4 + xs;
-        }
-        memcpy(b.names + names_used, fi->filename, nlen);
+        zx_find_sha(e, fi->extrafield, fi->extrafield ? fi->extrafield_size : 0);
+        memcpy(names + names_used, fi->filename, nlen);
         /* the compressed bytes, untouched, through the raw seam */
         if (csz) {
             err = mz_zip_entry_read_open(zip_handle, 1, NULL);
             size_t got = 0;
             while (err == MZ_OK && got < csz) {
                 const int32_t want = csz - got > (1u << 30) ? (int32_t)(1u << 30) : (int32_t)(csz - got);
-                const int32_t r = mz_zip_entry_read(zip_handle, b.h_comp + comp_used + got, want);
+                const int32_t r = mz_zip_entry_read(zip_handle, z.h_in + comp_used + got, want);
                 if (r <= 0) {
                     err = r < 0 ? r : MZ_READ_ERROR;
                     break;
@@ -1405,7 +1503,7 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
             if (err != MZ_OK)
                 break;
         }
-        memset(b.h_comp + comp_used + csz, 0, cneed - csz);
+        memset(z.h_in + comp_used + csz, 0, cneed - csz);
         comp_used += cneed;
         out_used += oneed;
         names_used += nlen;
@@ -1414,8 +1512,447 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
         err = mz_zip_goto_next_entry(zip_handle);
     }
     if (err == MZ_END_OF_LIST)
-        err = zx_flush(&b, n, comp_used, out_used, password, cb, userdata, &st);
-    zx_free(&b);
+        err = zx_flush(&z, ent, n, comp_used, names, password, cb, userdata, &st);
+    zr_free(&z);
+    free(ent);
+    free(names);
+    if (stats)
+        *stats = st;
+    return err;
+}
+
+/* ---- the native archive extractor (mz_zip_cuda_extract_archive) ---------------------------------------------------------- */
+static uint32_t get16(const uint8_t *p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
+static uint32_t get32(const uint8_t *p) { return get16(p) | (get16(p + 2) << 16); }
+static uint64_t get64(const uint8_t *p) { return (uint64_t)get32(p) | ((uint64_t)get32(p + 4) << 32); }
+
+static int32_t zn_seek(void *base, int64_t off) {
+    mz_stream *s = (mz_stream *)base;
+    if (!s || !s->vtbl || !s->vtbl->seek)
+        return MZ_PARAM_ERROR;
+    return s->vtbl->seek(s, off, MZ_SEEK_SET) == MZ_OK ? MZ_OK : MZ_SEEK_ERROR;
+}
+
+/* n bytes at absolute offset off, in reads of at most 1 GiB (the vtbl takes int32_t sizes) */
+static int32_t zn_read_at(void *base, int64_t off, uint8_t *p, uint64_t n) {
+    int32_t err = zn_seek(base, off);
+    while (err == MZ_OK && n > 0) {
+        const int32_t part = n > (1u << 30) ? (int32_t)(1u << 30) : (int32_t)n;
+        const int32_t r = mz_abi_base_read(base, p, part);
+        if (r <= 0)
+            return r < 0 ? r : MZ_READ_ERROR;
+        p += r;
+        n -= (uint64_t)r;
+    }
+    return err;
+}
+
+static int zn_cmp_off(const void *a, const void *b, void *ctx) {
+    const zx_entry *e = (const zx_entry *)ctx;
+    const uint64_t x = e[*(const uint32_t *)a].off, y = e[*(const uint32_t *)b].off;
+    return x < y ? -1 : x > y;
+}
+
+/* The central directory, read with one base read and parsed here (mz_zip.c:131-200 end records, :947-1100 directory and the
+ * correction for prepended data, :231 record layout): every entry's local-header offset, sizes, CRC, method, AES strength, expected
+ * SHA-256, name; then every entry's extent (its offset up to the next higher one or the directory). */
+static int32_t zn_read_directory(void *base, const char *password, zx_entry **out_ent, uint32_t *out_n, char **out_names, int32_t *out_refuse) {
+    int32_t err, refuse = MZ_OK;
+    int64_t size;
+    uint8_t *tail = NULL, *cd = NULL;
+    zx_entry *ent = NULL;
+    char *names = NULL;
+    *out_ent = NULL;
+    *out_names = NULL;
+    *out_n = 0;
+    *out_refuse = MZ_OK;
+    {
+        mz_stream *s = (mz_stream *)base;
+        if (!s || !s->vtbl || !s->vtbl->seek || !s->vtbl->tell || s->vtbl->seek(s, 0, MZ_SEEK_END) != MZ_OK)
+            return MZ_SEEK_ERROR;
+        size = s->vtbl->tell(s);
+        if (size < 0)
+            return MZ_TELL_ERROR;
+    }
+    /* the end record: the last signature within 64 KiB + 22 bytes of the end (mz_zip_search_eocd) */
+    const int64_t tl = size < 65535 + 22 ? size : 65535 + 22;
+    tail = (uint8_t *)malloc((size_t)tl + 1);
+    if (!tail)
+        return MZ_MEM_ERROR;
+    err = zn_read_at(base, size - tl, tail, (uint64_t)tl);
+    int64_t eocd = -1;
+    for (int64_t i = tl - 22; err == MZ_OK && i >= 0; i--)
+        if (get32(tail + i) == 0x06054b50u) {
+            eocd = size - tl + i;
+            break;
+        }
+    if (err == MZ_OK && eocd < 0)
+        err = MZ_FORMAT_ERROR;
+    uint64_t count = 0, cd_size = 0, cd_off = 0;
+    int64_t eocd_pos = eocd;
+    if (err == MZ_OK) {
+        const uint8_t *q = tail + (eocd - (size - tl));
+        const uint32_t disk = get16(q + 4), disk_cd = get16(q + 6), on_disk = get16(q + 8);
+        count = get16(q + 10);
+        cd_size = get32(q + 12);
+        cd_off = get32(q + 16);
+        if (disk != 0 || disk_cd != 0)
+            err = MZ_SUPPORT_ERROR; /* split archive */
+        else if (on_disk != count)
+            err = MZ_FORMAT_ERROR;
+        if (err == MZ_OK && (count == 0xffffu || cd_off == 0xffffffffu || cd_size == 0xffffffffu)) {
+            /* zip64: the locator in front of the end record names the zip64 end record (mz_zip_search_zip64_eocd); with prepended
+             * data the record sits right in front of the locator instead */
+            uint8_t loc[20], z64[56];
+            int found = 0;
+            if (eocd >= 20 && zn_read_at(base, eocd - 20, loc, 20) == MZ_OK && get32(loc) == 0x07064b50u) {
+                const uint64_t at[2] = {get64(loc + 8), (uint64_t)(eocd - 20 - 56)};
+                for (int k = 0; k < 2 && !found; k++)
+                    if (at[k] + 56 <= (uint64_t)eocd && zn_read_at(base, (int64_t)at[k], z64, 56) == MZ_OK && get32(z64) == 0x06064b50u) {
+                        found = 1;
+                        eocd_pos = (int64_t)at[k];
+                    }
+            }
+            if (found) {
+                if (get32(z64 + 16) != 0 || get32(z64 + 20) != 0)
+                    err = MZ_SUPPORT_ERROR;
+                else if (get64(z64 + 24) != get64(z64 + 32))
+                    err = MZ_FORMAT_ERROR;
+                count = get64(z64 + 32);
+                cd_size = get64(z64 + 40);
+                cd_off = get64(z64 + 48);
+                if ((int64_t)cd_size < 0 || (int64_t)cd_off < 0)
+                    err = MZ_FORMAT_ERROR;
+            } else if (count == 0xffffu || cd_off == 0xffffffffu) {
+                err = MZ_FORMAT_ERROR;
+            }
+        }
+    }
+    free(tail);
+    /* prepended data (self-extracting archives): when the directory is not where the end record says, it is right in front of the
+     * end record, and every recorded offset is off by the same shift (mz_zip.c:1066-1086) */
+    int64_t shift = 0;
+    if (err == MZ_OK) {
+        uint8_t sig[4];
+        if (cd_off > (uint64_t)eocd_pos || cd_size > (uint64_t)eocd_pos)
+            err = MZ_FORMAT_ERROR;
+        else if (cd_size && (zn_read_at(base, (int64_t)cd_off, sig, 4) != MZ_OK || get32(sig) != 0x02014b50u)) {
+            const int64_t alt = eocd_pos - (int64_t)cd_size;
+            if (zn_read_at(base, alt, sig, 4) == MZ_OK && get32(sig) == 0x02014b50u) {
+                shift = alt - (int64_t)cd_off;
+                cd_off = (uint64_t)alt;
+            } else {
+                err = MZ_FORMAT_ERROR;
+            }
+        }
+        if (err == MZ_OK && cd_off + cd_size > (uint64_t)eocd_pos)
+            cd_size = (uint64_t)eocd_pos - cd_off;
+    }
+    if (err == MZ_OK && cd_size / 46 < count)
+        err = MZ_FORMAT_ERROR;
+    if (err == MZ_OK) {
+        cd = (uint8_t *)malloc(cd_size + 1);
+        ent = (zx_entry *)malloc((size_t)(count ? count : 1) * sizeof(zx_entry));
+        names = (char *)malloc(cd_size + count + 1);
+        if (!cd || !ent || !names)
+            err = MZ_MEM_ERROR;
+    }
+    if (err == MZ_OK)
+        err = zn_read_at(base, (int64_t)cd_off, cd, cd_size);
+    uint32_t n = 0;
+    size_t nused = 0;
+    /* A record that is malformed or names an entry this call refuses ends the list: the entries in front of it are extracted,
+     * and then its error is returned -- what the reference's reader does when its walk reaches that entry. */
+    for (uint64_t p = 0; err == MZ_OK && refuse == MZ_OK && p < cd_size;) {
+        const uint8_t *h = cd + p;
+        if (cd_size - p < 46 || get32(h) != 0x02014b50u || n >= count) {
+            refuse = MZ_FORMAT_ERROR;
+            break;
+        }
+        const uint32_t flag = get16(h + 8), nlen = get16(h + 28), xlen = get16(h + 30), clen = get16(h + 32);
+        if (46ull + nlen + xlen + clen > cd_size - p) {
+            refuse = MZ_FORMAT_ERROR;
+            break;
+        }
+        zx_entry *e = &ent[n];
+        memset(e, 0, sizeof(*e));
+        uint32_t method = get16(h + 10);
+        e->crc = get32(h + 16);
+        e->csize = get32(h + 20);
+        e->usize = get32(h + 24);
+        e->off = get32(h + 42);
+        uint32_t disk = get16(h + 34), aes_method = 0;
+        const uint8_t *xf = h + 46 + nlen;
+        for (uint32_t xo = 0; xo + 4 <= xlen;) {
+            /* a field's length is clamped to what is left of the extra field, as mz_zip.c:321-322 does */
+            const uint32_t id = get16(xf + xo), xs = get16(xf + xo + 2), xn = xo + 4 + xs > xlen ? xlen - xo - 4 : xs;
+            const uint8_t *x = xf + xo + 4, *xe = x + xn;
+            /* MZ_ZIP_EXTENSION_ZIP64: the saturated fields, in this order (mz_zip.c:325-343) */
+            if (id == 0x0001) {
+                if (e->usize == 0xffffffffu && x + 8 <= xe) { e->usize = get64(x); x += 8; }
+                if (e->csize == 0xffffffffu && x + 8 <= xe) { e->csize = get64(x); x += 8; }
+                if (e->off == 0xffffffffu && x + 8 <= xe) { e->off = get64(x); x += 8; }
+                if (disk == 0xffffu && x + 4 <= xe) disk = get32(x);
+            } else if (id == 0x9901 && xn == 7) { /* WinZip AES: version, "AE", strength, real method (mz_zip.c:415-440) */
+                e->aes = x[4];
+                aes_method = get16(x + 5);
+                if (e->aes < 1 || e->aes > 3)
+                    e->aes = 0xff;
+            }
+            xo += 4 + xs;
+        }
+        zx_find_sha(e, xf, xlen);
+        const int enc = (flag & 1u) != 0;
+        if (enc && method == 99 && e->aes)
+            method = aes_method;
+        e->method = (uint16_t)method;
+        const uint64_t aes_over = enc && e->aes && e->aes != 0xff ? 4u * e->aes + 4u + 12u : 0u;
+        if (enc && e->aes && !password) {
+            refuse = MZ_PASSWORD_ERROR; /* encrypted and no password given */
+        } else if ((enc && (!e->aes || e->aes == 0xff || strlen(password) > 128 || e->csize < aes_over)) || (!enc && e->aes) ||
+                   (method != 0 && method != 8) || e->usize > (1ull << 30) || e->csize > (1ull << 30) || disk != 0) {
+            refuse = MZ_SUPPORT_ERROR; /* PKWARE-encrypted, another codec, too large for the batch path, or on another disk */
+        } else if (method == 0 && e->csize - aes_over != e->usize) {
+            refuse = MZ_FORMAT_ERROR;
+        } else {
+            e->off += (uint64_t)shift;
+            if (e->off + 30 > cd_off) /* the local header must lie in front of the directory */
+                refuse = MZ_FORMAT_ERROR;
+        }
+        if (refuse != MZ_OK)
+            break;
+        if (!enc)
+            e->aes = 0;
+        e->name_off = (uint32_t)nused;
+        memcpy(names + nused, h + 46, nlen);
+        names[nused + nlen] = 0;
+        nused += nlen + 1;
+        p += 46ull + nlen + xlen + clen;
+        n++;
+    }
+    free(cd);
+    if (err == MZ_OK && refuse == MZ_OK && n != count)
+        refuse = MZ_FORMAT_ERROR;
+    /* extents: up to the next higher local-header offset or the directory, and never more than a header, the data and a
+     * descriptor can take */
+    uint32_t *ord = err == MZ_OK ? (uint32_t *)malloc((size_t)(n ? n : 1) * 4) : NULL;
+    if (err == MZ_OK && !ord)
+        err = MZ_MEM_ERROR;
+    if (err == MZ_OK) {
+        for (uint32_t i = 0; i < n; i++)
+            ord[i] = i;
+        qsort_r(ord, n, 4, zn_cmp_off, ent);
+        for (uint32_t k = 0, j = 0; k < n; k++) {
+            zx_entry *e = &ent[ord[k]];
+            while (j < n && ent[ord[j]].off <= e->off)
+                j++;
+            const uint64_t end = j < n ? ent[ord[j]].off : cd_off;
+            const uint64_t cap = 30u + 65535u + 65535u + e->csize + 24u;
+            e->ext = end - e->off < cap ? end - e->off : cap;
+        }
+    }
+    free(ord);
+    if (err != MZ_OK) {
+        free(ent);
+        free(names);
+        return err;
+    }
+    *out_ent = ent;
+    *out_names = names;
+    *out_n = n;
+    *out_refuse = refuse;
+    return MZ_OK;
+}
+
+/* a round's stored bytes into z->h_in: extents in directory order, packed; one base read per run of adjacent extents */
+static int32_t zn_fill(zr_slot *z, void *base, const zx_entry *ent, uint64_t *src) {
+    int32_t err = MZ_OK;
+    size_t pos = 0, run_pos = 0;
+    uint64_t run_off = 0, run_len = 0;
+    for (uint32_t i = z->first; i < z->last && err == MZ_OK; i++) {
+        const zx_entry *e = &ent[i];
+        if (run_len && e->off != run_off + run_len) {
+            err = zn_read_at(base, (int64_t)run_off, z->h_in + run_pos, run_len);
+            run_len = 0;
+        }
+        if (!run_len) {
+            run_off = e->off;
+            run_pos = pos;
+        }
+        run_len += e->ext;
+        src[i - z->first] = pos;
+        pos += e->ext;
+    }
+    if (err == MZ_OK && run_len)
+        err = zn_read_at(base, (int64_t)run_off, z->h_in + run_pos, run_len);
+    memset(z->h_in + pos, 0, 64);
+    z->in_used = pos;
+    return err;
+}
+
+int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uint32_t flags, mz_cuda_zip_entry_cb cb, void *userdata,
+                                    mz_cuda_zip_stats *stats) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (!base_stream || (flags & ~MZ_ZIP_CUDA_ALL_DEVICES))
+        return MZ_PARAM_ERROR;
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    double t0 = now_ms();
+    zx_entry *ent = NULL;
+    char *names = NULL;
+    uint32_t count = 0;
+    int32_t refuse = MZ_OK;
+    int32_t err = zn_read_directory(base_stream, password, &ent, &count, &names, &refuse);
+    if (err) {
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    /* rounds: runs of entries in directory order whose extents fit the staging (32 MiB by default) and whose plain bytes fit four
+     * times that; an entry larger than a round gets a round of its own size */
+    size_t round_bytes = 32u << 20;
+    {
+        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
+        if (v && atoll(v) > 0)
+            round_bytes = (size_t)atoll(v) << 20;
+    }
+    const size_t out_round = round_bytes * 4;
+    uint32_t nrounds = 0, rcap = 16, max_ent = 1;
+    size_t max_in = 64, max_out = 64;
+    uint32_t *rfirst = (uint32_t *)malloc((rcap + 1) * sizeof(uint32_t));
+    uint64_t *src = NULL;
+    if (!rfirst)
+        err = MZ_MEM_ERROR;
+    for (uint32_t i = 0; i < count && err == MZ_OK;) {
+        size_t in = 0, out = 0;
+        uint32_t j = i;
+        while (j < count) {
+            const size_t oneed = ((size_t)ent[j].usize + 15) & ~(size_t)15;
+            if (j > i && (in + ent[j].ext > round_bytes || out + oneed > out_round))
+                break;
+            in += ent[j].ext;
+            out += oneed;
+            j++;
+        }
+        if (nrounds == rcap) {
+            uint32_t *q = (uint32_t *)realloc(rfirst, (rcap * 2 + 1) * sizeof(uint32_t));
+            if (!q) {
+                err = MZ_MEM_ERROR;
+                break;
+            }
+            rfirst = q;
+            rcap *= 2;
+        }
+        rfirst[nrounds++] = i;
+        if (in > max_in) max_in = in;
+        if (out > max_out) max_out = out;
+        if (j - i > max_ent) max_ent = j - i;
+        i = j;
+    }
+    if (err == MZ_OK) {
+        rfirst[nrounds] = count;
+        /* staging is pooled by capacity: round it up so that similar archives share it */
+        max_in = max_in > round_bytes ? (max_in + 65535) & ~(size_t)65535 : round_bytes;
+        max_out = max_out > out_round ? (max_out + 65535) & ~(size_t)65535 : out_round;
+        max_ent = (max_ent + 4095) & ~4095u;
+        src = (uint64_t *)malloc((size_t)max_ent * 8);
+        if (!src)
+            err = MZ_MEM_ERROR;
+    }
+    st.pack_ms += now_ms() - t0;
+    int32_t ndev = 1;
+    const int32_t dev0 = mz_cuda_get_device() < 0 ? 0 : mz_cuda_get_device();
+    if (flags & MZ_ZIP_CUDA_ALL_DEVICES) {
+        ndev = mz_cuda_device_count();
+        if (ndev < 1) ndev = 1;
+        if (ndev > 8) ndev = 8;
+    }
+    const double t_setup0 = now_ms();
+    /* an entry larger than a round makes every slot as large as it: then one slot per device, and it is not pooled */
+    const int oversized = max_in > round_bytes || max_out > out_round;
+    const uint32_t want = oversized ? (uint32_t)ndev : ndev > 1 ? (uint32_t)ndev * 2 : 4u;
+    const uint32_t nslots = want < nrounds ? want : (nrounds ? nrounds : 1);
+    zr_slot *slots = err == MZ_OK ? (zr_slot *)calloc(nslots, sizeof(zr_slot)) : NULL;
+    if (err == MZ_OK && !slots)
+        err = MZ_MEM_ERROR;
+    for (uint32_t k = 0; k < nslots && err == MZ_OK && nrounds; k++) {
+        const int32_t dev = ndev > 1 ? (int32_t)(k % (uint32_t)ndev) : dev0;
+        if (mz_cuda_set_device(dev) != MZ_OK || !zr_acquire(&slots[k], dev, max_in, max_out, max_ent))
+            err = MZ_MEM_ERROR;
+        slots[k].password = password;
+    }
+    mz_cuda_set_device(dev0);
+    st.setup_ms = now_ms() - t_setup0;
+    /* the caller's thread reads rounds ahead into free slots (the base stream is not thread-safe), each slot's worker runs the
+     * device work on its own stream, and finished rounds are delivered in archive order. A base read that fails while reading ahead
+     * stops the issuing; the rounds issued before it are still delivered, then its error is returned. */
+    uint32_t issued = 0, stop = nrounds;
+    int32_t read_err = MZ_OK;
+    for (uint32_t r = 0; r < stop && err == MZ_OK; r++) {
+        while (issued < stop && issued < r + nslots) {
+            zr_slot *z = &slots[issued % nslots];
+            const double t1 = now_ms();
+            z->first = rfirst[issued];
+            z->last = rfirst[issued + 1];
+            read_err = zn_fill(z, base_stream, ent, src);
+            if (read_err == MZ_OK)
+                zr_table(z, ent, z->first, z->last, src, 0);
+            st.pack_ms += now_ms() - t1;
+            if (read_err) {
+                stop = issued;
+                break;
+            }
+            z->running = pthread_create(&z->th, NULL, zr_run, z) == 0;
+            if (!z->running)
+                zr_run(z);
+            issued++;
+        }
+        if (r >= stop)
+            break;
+        zr_slot *z = &slots[r % nslots];
+        if (z->running) {
+            pthread_join(z->th, NULL);
+            z->running = 0;
+        }
+        err = z->err ? z->err : zr_verdict(z, 1);
+        if (err)
+            break;
+        const double t2 = now_ms();
+        err = zr_deliver(z, ent, names, cb, userdata, &st);
+        st.container_ms += now_ms() - t2;
+        st.gpu_ms += z->gpu_ms;
+        st.entries += z->n;
+        st.rounds++;
+    }
+    for (uint32_t k = 0; slots && k < nslots; k++)
+        if (slots[k].running) {
+            pthread_join(slots[k].th, NULL);
+            slots[k].running = 0;
+        }
+    if (err == MZ_OK)
+        err = read_err;
+    if (err == MZ_OK)
+        err = refuse; /* the entry that ended the list (zn_read_directory), after every entry in front of it was delivered */
+    const double t_setup1 = now_ms();
+    for (uint32_t k = 0; slots && k < nslots; k++) {
+        if (!slots[k].h_in)
+            continue;
+        mz_cuda_set_device(slots[k].device);
+        if (oversized)
+            zr_free(&slots[k]);
+        else
+            zr_release(&slots[k]);
+    }
+    mz_cuda_set_device(dev0);
+    st.setup_ms += now_ms() - t_setup1;
+    free(slots);
+    free(src);
+    free(rfirst);
+    free(ent);
+    free(names);
     if (stats)
         *stats = st;
     return err;
