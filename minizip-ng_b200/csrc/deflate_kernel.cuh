@@ -202,6 +202,38 @@ __device__ inline uint32_t block_excl_sum(uint32_t v, uint32_t *scan, uint32_t &
     return res;
 }
 
+/* ---- opt-in per-phase cycle counters (compile with -DMZ_DF_PHASES: `make phases`, read by tools/deflate_phases.py) ---------------
+ * Thread 0 of every CTA reads clock64() right after the barrier that ends a phase and adds the cycles since its previous reading to
+ * column `phase` of the CTA's row of g_df_phases (column DF_PH_UNITS counts the units). After a barrier every thread of the CTA is
+ * done with the phase before, so the deltas are the CTA's wall time per phase; no barrier is added. Inside D the same marks split
+ * the phase at its named barriers (thread 0 takes part in D) into the DF_PH_D_* columns, whose sum is at most D's; the rest of D
+ * is the header. DF_PH_D_PASSES + n counts the units whose Kraft completion ran n passes (the last bucket: 7 or more). Without the
+ * macro (the product library) and on the emulator the marks compile to nothing. */
+enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_E_SCAN, DF_PH_F_M3, DF_PH_FLUSH, DF_PH_UNITS,
+       DF_PH_D_STATS, DF_PH_D_SWEEP1, DF_PH_D_SWEEP2, DF_PH_D_KRAFT, DF_PH_D_CANON, DF_PH_D_PASSES, DF_PH_COLS = DF_PH_D_PASSES + 8 };
+constexpr int DF_PH_ROWS = 1024;
+#if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
+__device__ unsigned long long g_df_phases[DF_PH_ROWS][DF_PH_COLS];
+#define DF_PHASE_BEGIN(t) unsigned long long t = clock64()
+#define DF_PHASE(t, ph)                                                                        \
+    do {                                                                                       \
+        if (threadIdx.x == 0 && blockIdx.x < (unsigned)DF_PH_ROWS) {                           \
+            const unsigned long long now_ = clock64();                                         \
+            atomicAdd(&g_df_phases[blockIdx.x][ph], now_ - (t));                               \
+            if ((ph) == DF_PH_LOAD) atomicAdd(&g_df_phases[blockIdx.x][DF_PH_UNITS], 1ull);   \
+            (t) = now_;                                                                        \
+        }                                                                                      \
+    } while (0)
+#define DF_PHASE_COUNT(col)                                                                                          \
+    do {                                                                                                             \
+        if (threadIdx.x == 0 && blockIdx.x < (unsigned)DF_PH_ROWS) atomicAdd(&g_df_phases[blockIdx.x][col], 1ull); \
+    } while (0)
+#else
+#define DF_PHASE_BEGIN(t)
+#define DF_PHASE(t, ph)
+#define DF_PHASE_COUNT(col)
+#endif
+
 /* ---- D: block-parallel literal/length + distance codes ------------------------------------------------
  * Thread i < 288 owns literal/length symbol i (286 used), thread 288 + j owns distance symbol j (30 used);
  * both alphabets are warp aligned (warps 0-8 and warp 9). Called by threads 0..319 ONLY; they synchronise
@@ -209,8 +241,8 @@ __device__ inline uint32_t block_excl_sum(uint32_t v, uint32_t *scan, uint32_t &
  * bb = 512 words of shared scratch. Outputs lens (u8), codes (reversed code | len << 16 | extra bits << 20)
  * and bits (u8: code length + extra bits = what one entry of that symbol costs). */
 constexpr int DF_BB_THREADS = 320;
-enum { BB_STAT = 0 /* [2][4]: used,total,first */, BB_KRAFT = 8 /* [2 sweeps][2 alph][16] */, BB_K = 72 /* [2][16] */,
-       BB_NEXT = 104 /* [2][16] */, BB_SLACK = 136 /* [2] */, BB_CNTW = 144 /* [2 bufs][10 warps][16] */,
+enum { BB_STAT = 0 /* [2][4]: used,total,first */, BB_KRAFT = 8 /* [2 sweeps][2 alph][16] */, BB_SLACK = 136 /* [2] */,
+       BB_CNTW = 144 /* [2 bufs][10 warps][16]: codes per length in a warp, then what a code's rank in its warp is set against */,
        BB_NZ = 464 /* [10] ballots: length != 0 */, BB_ST = 474 /* [10] ballots: a run of equal lengths starts here */,
        BB_HSUM = 484 /* [10] header bits per warp */, BB_HDRBITS = 494 /* size of the block header in bits */ };
 
@@ -249,6 +281,7 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
     const uint32_t one = 1u << M;
     const uint32_t w0 = a == 0 ? 0u : 9u; /* first warp of my alphabet */
     uint32_t c = (a < 2 && sym < nsym) ? (a == 0 ? hist_ll[sym] + (sym < 256 ? hist_lit2[sym] : 0u) : hist_d[sym]) : 0u;
+    DF_PHASE_BEGIN(d_t);
 
     if (tid < 144) bb[tid] = (tid == BB_STAT + 2 || tid == BB_STAT + 6) ? 0xffffffffu : 0u;
     bar_sync(1, DF_BB_THREADS);
@@ -263,6 +296,7 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
         }
     }
     bar_sync(1, DF_BB_THREADS);
+    DF_PHASE(d_t, DF_PH_D_STATS);
     float ideal = 0.f;
     if (a < 2) {
         uint32_t used = bb[BB_STAT + a * 4 + 0], total = bb[BB_STAT + a * 4 + 1], fu = bb[BB_STAT + a * 4 + 2];
@@ -279,6 +313,7 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
     uint32_t slack[2] = {0, 0};
     for (int sweep = 0; sweep < 2; sweep++) {
         if (a < 2) {
+            uint32_t mine = 0; /* lane cnd < 16 keeps the warp's Kraft sum for candidate cnd */
 #pragma unroll
             for (int cnd = 0; cnd < 16; cnd++) {
                 uint32_t kr = 0;
@@ -288,21 +323,25 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
                     kr = 1u << (M - l);
                 }
                 kr = __reduce_add_sync(MZ_FULL_MASK, kr);
-                if (lane == 0) atomicAdd(&bb[BB_KRAFT + sweep * 32 + a * 16 + cnd], kr);
+                mine = lane == (unsigned)cnd ? kr : mine;
             }
+            if (lane < 16) atomicAdd(&bb[BB_KRAFT + sweep * 32 + a * 16 + lane], mine); /* one shared atomic per warp and sweep */
         }
         bar_sync(1, DF_BB_THREADS);
-        /* everyone derives both alphabets' choices (uniform): the largest feasible candidate */
-        float lo_a = lo;
-        for (int aa = 0; aa < 2; aa++) {
-            int best = 0;
-            for (int cnd = 1; cnd < 16; cnd++)
-                if (bb[BB_KRAFT + sweep * 32 + aa * 16 + cnd] <= one) best = cnd;
-            slack[aa] = one - bb[BB_KRAFT + sweep * 32 + aa * 16 + best];
-            if (aa == a) lo_a = lo + step * (float)best;
-        }
+        DF_PHASE(d_t, DF_PH_D_SWEEP1 + sweep);
+        /* Every warp derives both alphabets' choices (uniform): the largest candidate in 1..15 whose Kraft sum is at most 1, else
+         * 0. Lane l holds the sum of candidate l & 15 of alphabet l >> 4, so a ballot of "fits" and its highest bit per half give
+         * the same `best` as scanning the candidates upwards and keeping the last that fits -- whatever the order of the sums.
+         * (They do not decrease with the candidate anyway: lo + step * cnd is an exact binary fraction that grows with cnd, so
+         * every length only shrinks.) */
+        const uint32_t kl = bb[BB_KRAFT + sweep * 32 + lane];
+        const unsigned fit = __ballot_sync(MZ_FULL_MASK, (lane & 15u) != 0 && kl <= one);
+        const int best0 = (fit & 0xffffu) ? 31 - __clz((int)(fit & 0xffffu)) : 0;
+        const int best1 = (fit >> 16) ? 31 - __clz((int)(fit >> 16)) : 0;
+        slack[0] = one - __shfl_sync(MZ_FULL_MASK, kl, best0);
+        slack[1] = one - __shfl_sync(MZ_FULL_MASK, kl, 16 + best1);
         /* lo is per alphabet from here on; the loop variable is private to the thread */
-        lo = lo_a;
+        lo = lo + step * (float)(a == 0 ? best0 : best1);
         step *= 0.0625f;
     }
     uint32_t L = 0;
@@ -310,20 +349,28 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
         int l = (int)ceilf(ideal - lo);
         L = (uint32_t)(l < 1 ? 1 : (l > M ? M : l));
     }
-    /* exact Kraft completion: shorten codes (short ones first) until the sum is exactly 1 */
+    /* exact Kraft completion: shorten codes (short ones first) until the sum is exactly 1. A pass that leaves no slack in either
+     * alphabet also lays out the canonical codes (below), so the usual case -- one pass -- needs no second count and no more
+     * barriers. */
     unsigned m = 0;
-    int buf = 0;
-    for (int pass = 0; pass < 40; pass++) {
+    int buf = 0, pass = 0;
+    bool settled = false;
+    for (; pass < 40; pass++) {
         if (slack[0] == 0 && slack[1] == 0) break;
-        uint32_t *cntw = bb + BB_CNTW + buf * 160;
+        uint32_t *cntw = bb + BB_CNTW + buf * 160, *nxt = bb + BB_CNTW + (buf ^ 1) * 160;
         if (a < 2) bb_count_lengths(cntw + w * 16, L, lane, m);
         bar_sync(1, DF_BB_THREADS);
         if (w == 0 || w == 9) { /* one warp per alphabet: lane = code length; the recurrence over lengths is uniform */
             const int aa = w == 0 ? 0 : 1;
             const uint32_t wa = aa == 0 ? 0u : 9u, wb = aa == 0 ? 9u : 10u;
-            uint32_t tot = 0;
-            if (lane >= 2 && lane <= (unsigned)M)
-                for (uint32_t ww = wa; ww < wb; ww++) tot += cntw[ww * 16 + lane];
+            const bool mine = lane >= 1 && lane <= (unsigned)M;
+            uint32_t P[9], tot = 0; /* P[i] = the count in the warps before warp wa + i (all nine loads in flight at once) */
+#pragma unroll
+            for (int i = 0; i < 9; i++) {
+                const uint32_t t = (mine && wa + i < wb) ? cntw[(wa + i) * 16 + lane] : 0u;
+                P[i] = tot;
+                tot += t;
+            }
             uint32_t sl = slack[aa], myk = 0;
             for (int len = 2; len <= M; len++) {
                 uint32_t t = __shfl_sync(MZ_FULL_MASK, tot, len);
@@ -332,44 +379,80 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
                 if (lane == (unsigned)len) myk = k;
                 sl -= k << (M - len);
             }
-            if (lane >= 2 && lane <= (unsigned)M) bb[BB_K + aa * 16 + lane] = myk;
+            /* The codes per length after this pass: k[len] leave length len, k[len + 1] arrive from len + 1. Their canonical first
+             * codes, in case this pass is the last. */
+            const uint32_t kup = __shfl_down_sync(MZ_FULL_MASK, myk, 1);
+            const uint32_t tot2 = mine ? tot - myk + kup : 0u;
+            uint32_t code = 0, prev = 0, mycode = 0;
+            for (int len = 1; len <= M; len++) {
+                code = (code + prev) << 1;
+                if (lane == (unsigned)len) mycode = code;
+                prev = __shfl_sync(MZ_FULL_MASK, tot2, len);
+            }
+            /* Per warp ww and length: k - P (a code of that length in warp ww whose rank in its warp is below it is one of the
+             * first k of its length in symbol order, the ones to shorten), and into the other buffer the first code of the length
+             * after the pass + the codes of that length in the warps before ww after the pass: P - min(k, P) that stay and
+             * min(k[len + 1], P[len + 1]) that arrive. */
+#pragma unroll
+            for (int i = 0; i < 9; i++) {
+                const uint32_t Pup = __shfl_down_sync(MZ_FULL_MASK, P[i], 1);
+                if (mine && wa + i < wb) {
+                    cntw[(wa + i) * 16 + lane] = myk - P[i];
+                    nxt[(wa + i) * 16 + lane] = mycode + P[i] - (myk < P[i] ? myk : P[i]) + (kup < Pup ? kup : Pup);
+                }
+            }
             if (lane == 0) bb[BB_SLACK + aa] = sl;
         }
         bar_sync(1, DF_BB_THREADS);
         if (a < 2 && L >= 2) {
-            uint32_t rank = (uint32_t)__popc(m & ((1u << lane) - 1));
-            for (uint32_t ww = w0; ww < w; ww++) rank += cntw[ww * 16 + L];
-            if (rank < bb[BB_K + a * 16 + L]) L -= 1;
+            const int rank = __popc(m & ((1u << lane) - 1));
+            if (rank < (int)cntw[w * 16 + L]) L -= 1;
         }
         slack[0] = bb[BB_SLACK + 0];
         slack[1] = bb[BB_SLACK + 1];
         buf ^= 1;
-    }
-    /* canonical codes: code = first code of its length + rank among equal lengths in symbol order */
-    uint32_t *cntw = bb + BB_CNTW + buf * 160;
-    if (a < 2) bb_count_lengths(cntw + w * 16, L, lane, m);
-    bar_sync(1, DF_BB_THREADS);
-    if (w == 0 || w == 9) {
-        const int aa = w == 0 ? 0 : 1;
-        const uint32_t wa = aa == 0 ? 0u : 9u, wb = aa == 0 ? 9u : 10u;
-        uint32_t tot = 0;
-        if (lane >= 1 && lane <= (unsigned)M)
-            for (uint32_t ww = wa; ww < wb; ww++) tot += cntw[ww * 16 + lane];
-        uint32_t code = 0, prev = 0, mycode = 0;
-        for (int len = 1; len <= M; len++) {
-            code = (code + prev) << 1;
-            if (lane == (unsigned)len) mycode = code;
-            prev = __shfl_sync(MZ_FULL_MASK, tot, len);
+        if (slack[0] == 0 && slack[1] == 0) {
+            settled = true;
+            pass++;
+            break;
         }
-        if (lane >= 1 && lane <= (unsigned)M) bb[BB_NEXT + aa * 16 + lane] = mycode;
     }
-    bar_sync(1, DF_BB_THREADS);
+    DF_PHASE(d_t, DF_PH_D_KRAFT);
+    DF_PHASE_COUNT(DF_PH_D_PASSES + (pass < 7 ? pass : 7));
+    /* canonical codes: code = first code of its length + rank among equal lengths in symbol order; the rows of cntw hold the
+     * first code + the count in the warps before */
+    uint32_t *cntw = bb + BB_CNTW + buf * 160;
+    if (settled) { /* laid out by the last pass; only the rank in the warp is left */
+        if (a < 2) m = __match_any_sync(MZ_FULL_MASK, L);
+    } else { /* no pass ran, or none left both alphabets without slack */
+        if (a < 2) bb_count_lengths(cntw + w * 16, L, lane, m);
+        bar_sync(1, DF_BB_THREADS);
+        if (w == 0 || w == 9) {
+            const int aa = w == 0 ? 0 : 1;
+            const uint32_t wa = aa == 0 ? 0u : 9u, wb = aa == 0 ? 9u : 10u;
+            const bool mine = lane >= 1 && lane <= (unsigned)M;
+            uint32_t tot = 0;
+            if (mine)
+                for (uint32_t ww = wa; ww < wb; ww++) {
+                    const uint32_t t = cntw[ww * 16 + lane];
+                    cntw[ww * 16 + lane] = tot;
+                    tot += t;
+                }
+            uint32_t code = 0, prev = 0, mycode = 0;
+            for (int len = 1; len <= M; len++) {
+                code = (code + prev) << 1;
+                if (lane == (unsigned)len) mycode = code;
+                prev = __shfl_sync(MZ_FULL_MASK, tot, len);
+            }
+            if (mine)
+                for (uint32_t ww = wa; ww < wb; ww++) cntw[ww * 16 + lane] += mycode;
+        }
+        bar_sync(1, DF_BB_THREADS);
+    }
     if (a < 2) {
         uint32_t cw = 0;
         if (L) {
-            uint32_t rank = (uint32_t)__popc(m & ((1u << lane) - 1));
-            for (uint32_t ww = w0; ww < w; ww++) rank += cntw[ww * 16 + L];
-            uint32_t code = bb[BB_NEXT + a * 16 + L] + rank;
+            const uint32_t code = cntw[w * 16 + L] + (uint32_t)__popc(m & ((1u << lane) - 1));
             cw = (__brev(code) >> (32 - L)) | (L << 16);
         }
         if (a == 0) {
@@ -389,6 +472,7 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
     const unsigned nz = __ballot_sync(MZ_FULL_MASK, L != 0);
     if (lane == 0) bb[BB_NZ + w] = nz;
     bar_sync(1, DF_BB_THREADS);
+    DF_PHASE(d_t, DF_PH_D_CANON);
     const uint32_t hlit = 256u + 32u - (uint32_t)__clz((int)bb[BB_NZ + 8]); /* the end-of-block symbol always has a code: >= 257 */
     const uint32_t hdw = bb[BB_NZ + 9];
     const uint32_t hdist = hdw ? 32u - (uint32_t)__clz((int)hdw) : 1u;
@@ -574,30 +658,6 @@ __device__ __forceinline__ uint32_t nth_parked(const uint32_t (&bm)[DF_NBATCH], 
     }
     return found ? bsel * (uint32_t)DF_THREADS + warp * 32u + base : 0xffffffffu;
 }
-
-/* ---- opt-in per-phase cycle counters (compile with -DMZ_DF_PHASES: `make phases`, read by tools/deflate_phases.py) ---------------
- * Thread 0 of every CTA reads clock64() right after the barrier that ends a phase and adds the cycles since its previous reading to
- * column `phase` of the CTA's row of g_df_phases (column DF_PH_UNITS counts the units). After a barrier every thread of the CTA is
- * done with the phase before, so the deltas are the CTA's wall time per phase; no barrier is added. Without the macro (the product
- * library) and on the emulator the marks compile to nothing. */
-enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_E_SCAN, DF_PH_F_M3, DF_PH_FLUSH, DF_PH_UNITS, DF_PH_COLS };
-constexpr int DF_PH_ROWS = 1024;
-#if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
-__device__ unsigned long long g_df_phases[DF_PH_ROWS][DF_PH_COLS];
-#define DF_PHASE_BEGIN(t) unsigned long long t = clock64()
-#define DF_PHASE(t, ph)                                                                        \
-    do {                                                                                       \
-        if (threadIdx.x == 0 && blockIdx.x < (unsigned)DF_PH_ROWS) {                           \
-            const unsigned long long now_ = clock64();                                         \
-            atomicAdd(&g_df_phases[blockIdx.x][ph], now_ - (t));                               \
-            if ((ph) == DF_PH_LOAD) atomicAdd(&g_df_phases[blockIdx.x][DF_PH_UNITS], 1ull);   \
-            (t) = now_;                                                                        \
-        }                                                                                      \
-    } while (0)
-#else
-#define DF_PHASE_BEGIN(t)
-#define DF_PHASE(t, ph)
-#endif
 
 /* ---- the kernel ------------------------------------------------------------------------------- */
 template <int STRIDE, bool LAZY, bool HIST = false>
@@ -1095,6 +1155,9 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 __syncthreads(); /* S4 */
                 DF_PHASE(ph_t, DF_PH_T_M1);
                 /* ---- D: codes (10 warps on a named barrier; the rest wait here) ------------------------- */
+#ifdef MZ_DF_CODES_HOOK /* test builds only (tests/emu/emu_df_codes.cc): record the histograms the builder is given */
+                if (tid == 0) MZ_DF_CODES_HOOK(s_hist_ll, (const uint32_t *)(smem + DF_OFF_HIST2), s_hist_d);
+#endif
                 if (tid < DF_BB_THREADS)
                     block_build_codes(s_hist_ll, (const uint32_t *)(smem + DF_OFF_HIST2), s_hist_d, s_lens_ll, s_lens_d, s_code_ll, s_code_d, s_bits_ll, s_bits_d, s_bb,
                                       s_stage, bitpos, bfinal);

@@ -2,7 +2,8 @@
 """Where the deflate kernel's cycles go, per phase, on the GPU: runs the instrumented library (minizip-ng_b200/
 libmz_strm_cuda_phases.so, built by `make -C minizip-ng_b200/csrc phases`: deflate_kernel.cuh with -DMZ_DF_PHASES) on the bench
 text with the C5 launch (64 KiB chunks, one launch over the whole buffer, 2 CTAs per SM) and prints SM cycles per 32 KiB unit
-and each phase's share, with the GPU's name, power limit and SM clock.
+and each phase's share, with the GPU's name, power limit and SM clock. D (the code construction) is split further at its named
+barriers: stats, the two sweeps, Kraft completion (with the number of units per pass count), canonical codes, and the header.
 
 The counters are thread 0's clock64() readings at the kernel's barriers, summed per CTA; cycles per unit = all CTAs' cycles over
 all units. The counting itself costs a few atomics per unit, so the kernel time printed here is not the product's.
@@ -18,7 +19,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 PHASES = ["load + hash reset", "parse batches", "M0", "cover", "T + M1", "D (codes + header)", "E + scan", "F + M3", "flush"]
-COLS = len(PHASES) + 1  # + units
+UNITS = len(PHASES)  # column layout of g_df_phases (deflate_kernel.cuh): the phases, the unit count, D's sub-phases, the pass counts
+D_SUB = ["stats", "sweep 1", "sweep 2", "Kraft completion", "canonical codes"]  # + "header": the rest of D
+D_COL = PHASES.index("D (codes + header)")
+NPASS = 8  # units whose Kraft completion ran 0, 1, .. 6, 7 or more passes
+COLS = UNITS + 1 + len(D_SUB) + NPASS
 ROWS = 1024
 
 
@@ -80,16 +85,22 @@ def main():
     kms = ev0.elapsed_time(ev1) / args.reps
     pkg.check(lib.mz_cuda_deflate_phases(rows, ROWS), "phases")
     tab = [[rows[r * COLS + c] for c in range(COLS)] for r in range(ROWS)]
-    tab = [r for r in tab if r[-1]]
-    units = sum(r[-1] for r in tab)
+    tab = [r for r in tab if r[UNITS]]
+    units = sum(r[UNITS] for r in tab)
     per = [sum(r[c] for r in tab) for c in range(len(PHASES))]
     total = sum(per)
-    busiest = max(sum(r[:-1]) for r in tab) / args.reps  # a CTA's cycles over the launch ~ kernel time x SM clock
+    busiest = max(sum(r[:UNITS]) for r in tab) / args.reps
+    dsub = [sum(r[UNITS + 1 + i] for r in tab) for i in range(len(D_SUB))]
+    dsub.append(per[D_COL] - sum(dsub))
+    passes = [sum(r[UNITS + 1 + len(D_SUB) + i] for r in tab) // args.reps for i in range(NPASS)]  # a CTA's cycles over the launch ~ kernel time x SM clock
     res = {"gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock_after": info.get("clocks.sm"),
            "sm_clock_max": info.get("clocks.max.sm"), "level": args.level, "bytes": n, "ctas": len(tab), "units": units // args.reps,
            "kernel_ms": round(kms, 3), "input_GBps": round(n / kms / 1e6, 1), "effective_sm_MHz": round(busiest / (kms * 1e3), 0),
            "ratio": round(int(out_len.sum().item()) / n, 4), "cycles_per_unit": round(total / units, 0),
-           "phases": {p: {"cycles_per_unit": round(c / units, 0), "share": round(c / total, 4)} for p, c in zip(PHASES, per)}}
+           "phases": {p: {"cycles_per_unit": round(c / units, 0), "share": round(c / total, 4)} for p, c in zip(PHASES, per)},
+           "d_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_d": round(c / max(per[D_COL], 1), 4)}
+                           for p, c in zip(D_SUB + ["header"], dsub)},
+           "kraft_passes": {("%d+" % i if i == NPASS - 1 else str(i)): n for i, n in enumerate(passes)}}
     print("%s, power limit %s, SM clock %s (max %s); effective clock during the launches %d MHz" % (
         res["gpu"], res["power_limit"], res["sm_clock_after"], res["sm_clock_max"], res["effective_sm_MHz"]))
     print("level %d, %.2f GiB of bench text, 64 KiB chunks, %d CTAs, %d units: %.3f ms per launch (instrumented), ratio %.4f" % (
@@ -97,7 +108,11 @@ def main():
     print("%-20s %12s %7s" % ("phase", "cycles/unit", "share"))
     for p, c in zip(PHASES, per):
         print("%-20s %12.0f %6.1f%%" % (p, c / units, 100.0 * c / total))
+        if p == PHASES[D_COL]:
+            for q, d in zip(D_SUB + ["header"], dsub):
+                print("  %-18s %12.0f %6.1f%% of D" % (q, d / units, 100.0 * d / max(per[D_COL], 1)))
     print("%-20s %12.0f" % ("total", total / units))
+    print("units by Kraft completion passes: " + ", ".join("%s: %d" % kv for kv in res["kraft_passes"].items()))
     print(json.dumps(res))
     if args.json:
         with open(args.json, "w") as f:
