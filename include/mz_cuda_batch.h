@@ -214,6 +214,33 @@ int32_t mz_cuda_zip_locate(const mz_cuda_zip_round *round, void *stream);
 int32_t mz_cuda_zip_copy_stored(const mz_cuda_zip_round *round, void *stream);
 int32_t mz_cuda_zip_verify(const mz_cuda_zip_round *round, void *stream);
 
+/* ---- K10: the central directory of an archive in device memory (csrc/zipcd_kernel.cuh) --------------------------------
+ * The parse behind mz_zip_cuda_extract_device (include/mz_zip_cuda.h): end records, the record chain from the directory's first
+ * record, each record's fields and refusal rules, extents and the output layout, all on the device; only a few scalars come back
+ * (it synchronises on `stream` between its stages). On return: err = an error of the archive as a whole (then nothing else is
+ * set); count = records accepted, refuse = the error of the record that ended the list (MZ_OK if none); the totals. The
+ * tables fit when max_entries >= count and, with `decode` set, out_cap >= out_bytes; otherwise nothing more is written. When they
+ * fit, `entries` (if not NULL) is filled (mz_cuda_zip_dev_entry, status 0) and, with `decode` set, `ent` (count K9 records: src_off = local header in the archive, src_len =
+ * extent) and `sha_expect` (nsha expected digests, 32 bytes each, the K9 sha_slot rows) are allocated on the device and filled;
+ * the caller frees them with mz_cuda_free. The function's own return value is MZ_OK or a CUDA / memory error. */
+typedef struct mz_cuda_zip_dir {
+    /* in */
+    uint32_t have_password, password_long; /* a password was given; it is longer than 128 bytes */
+    void *entries;                         /* device table of mz_cuda_zip_dev_entry, or NULL */
+    uint32_t max_entries, decode;
+    uint64_t out_cap;
+    /* out */
+    int32_t err, refuse;
+    uint32_t count, njobs, nsha, na[4], pad; /* na[s]: entries of WinZip AES strength s */
+    uint64_t cd_off, out_bytes, bytes_in, bytes_out, max_clen[4];
+    mz_cuda_zip_ent *ent;
+    void *sha_expect;
+} mz_cuda_zip_dir;
+int32_t mz_cuda_zip_parse_directory(const void *d_archive, uint64_t len, mz_cuda_zip_dir *dir, void *stream);
+/* after mz_cuda_zip_verify: each entry's status (0 or -MZ code) into the mz_cuda_zip_dev_entry table, and *d_first lowered to the
+ * index of the first failing entry (the caller sets it to 0xffffffff first) */
+int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entries, uint32_t *d_first, void *stream);
+
 /* ---- K6: one long foreign stream, segment-speculative (csrc/inflate_spec_kernel.cuh) ------------------------
  * One ROUND decodes as much of the compressed window d_in[0..in_avail) as can be proven, starting at the block
  * boundary `start_bit` (absolute bit; the serial decoder's state must be at a block header), into

@@ -130,6 +130,43 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
 int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uint32_t flags, mz_cuda_zip_entry_cb cb, void *userdata,
                                     mz_cuda_zip_stats *stats);
 
+/* ---- an archive in device memory, extracted into device memory ------------------------------------------------------
+ * The same extraction as mz_zip_cuda_extract_archive for an archive that already lies in device memory (d_archive, len bytes,
+ * current device; no padding needed): the central directory is parsed on the device (K10), every accepted entry is decoded and
+ * verified there (K9, K8, K5, K1, K7), and the plain bytes stay in device memory. Only a few scalars cross PCIe. Synchronous: the
+ * work is enqueued on `stream` and the call synchronises on it before it returns. The archive is not modified (WinZip AES entries
+ * are decrypted in a copy of the bytes in front of the directory).
+ * Results and errors are those of mz_zip_cuda_extract_archive on the same bytes:
+ *   - an error of the archive as a whole (end records, zip64 records, directory location, split archive) is returned first, with
+ *     *count = 0 and nothing decoded;
+ *   - *count = the directory records accepted; a refused record ends the list, the entries in front of it are decoded, then its
+ *     error is returned; *out_bytes = the plain bytes of the accepted entries, each rounded up to 16;
+ *   - d_out == NULL: list only: the table and *out_bytes are filled, nothing is decoded;
+ *   - max_entries < *count, or d_out and out_cap < *out_bytes: MZ_BUF_ERROR with *count and *out_bytes set, nothing decoded or
+ *     listed (call again with buffers that large; d_entries may be NULL with max_entries 0 for the first call). A truncated
+ *     stream is also MZ_BUF_ERROR, as an entry's error: the caps then cover *count and *out_bytes;
+ *   - otherwise every accepted entry is decoded and verified: local header, AES verifier and HMAC, DEFLATE end state and sizes,
+ *     CRC-32, SHA-256. The first failing entry in directory order decides the return value; each entry's status is in the table.
+ * A central directory of 16 GiB or more returns MZ_SUPPORT_ERROR (the device parse counts candidate records in 32 bits).
+ * d_entries: device table, one row per accepted record in directory order. d_out: 16-byte aligned. stats (may be NULL):
+ * entries / bytes_in / bytes_out of the accepted entries, pack_ms = the directory parse, gpu_ms = decode and verify, setup_ms =
+ * scratch allocation; rounds = 1 when something was decoded. */
+typedef struct mz_cuda_zip_dev_entry {
+    uint64_t local_off; /* local header in the archive, after the prepended-data shift */
+    uint64_t csize, usize;
+    uint64_t out_off;   /* plain bytes at d_out + out_off: 16-byte aligned, packed in directory order */
+    uint64_t name_off;  /* name bytes at d_archive + name_off (inside the central directory), name_len of them, not terminated */
+    uint64_t extent;    /* bytes from local_off up to the next local header or the directory (capped) */
+    uint64_t sha_off;   /* has_sha: the expected SHA-256 at d_archive + sha_off */
+    uint32_t crc, name_len;
+    uint16_t method;    /* 0 or 8 (an AES entry's real method) */
+    uint8_t aes;        /* 0 or WinZip AES strength 1..3 */
+    uint8_t has_sha;
+    int32_t status;     /* after decoding: MZ_OK or this entry's error */
+} mz_cuda_zip_dev_entry; /* 72 bytes */
+int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
+                                   uint32_t *count, void *d_out, uint64_t out_cap, uint64_t *out_bytes, mz_cuda_zip_stats *stats, void *stream);
+
 /* sizeof the mz_zip_file mirror this library was built with: the host asserts it equals sizeof(mz_zip_file) */
 uint32_t mz_zip_cuda_abi_file_info_size(void);
 

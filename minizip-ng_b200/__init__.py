@@ -58,9 +58,9 @@ EXPORTS = [
     "mz_cuda_stream_wait_event", "mz_cuda_gather", "mz_cuda_scatter_blobs",
     # include/mz_zip_cuda.h
     "mz_zip_cuda_add_buffers", "mz_zip_cuda_add_buffers_ex", "mz_zip_cuda_write_archive", "mz_zip_cuda_trim", "mz_zip_cuda_write_archive_aes", "mz_zip_cuda_extract_all",
-    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_abi_file_info_size",
-    # include/mz_cuda_batch.h, K9
-    "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify",
+    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_extract_device", "mz_zip_cuda_abi_file_info_size",
+    # include/mz_cuda_batch.h, K9 and K10
+    "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify", "mz_cuda_zip_parse_directory", "mz_cuda_zip_statuses",
 ]
 
 # mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
@@ -72,6 +72,13 @@ class ZipStats(C.Structure):
     """mz_cuda_zip_stats (include/mz_zip_cuda.h)"""
     _fields_ = [("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64), ("entries", C.c_uint32), ("rounds", C.c_uint32),
                 ("pack_ms", C.c_double), ("gpu_ms", C.c_double), ("container_ms", C.c_double), ("setup_ms", C.c_double)]
+
+
+class ZipDevEntry(C.Structure):
+    """mz_cuda_zip_dev_entry (include/mz_zip_cuda.h)"""
+    _fields_ = [("local_off", C.c_uint64), ("csize", C.c_uint64), ("usize", C.c_uint64), ("out_off", C.c_uint64), ("name_off", C.c_uint64),
+                ("extent", C.c_uint64), ("sha_off", C.c_uint64), ("crc", C.c_uint32), ("name_len", C.c_uint32), ("method", C.c_uint16),
+                ("aes", C.c_uint8), ("has_sha", C.c_uint8), ("status", C.c_int32)]
 
 
 class ZipItem(C.Structure):
@@ -166,6 +173,9 @@ def configure(L):
     sig("mz_zip_cuda_write_archive_aes", i32, [vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp])
     sig("mz_zip_cuda_extract_archive", i32, [vp, C.c_char_p, u32, ZIP_ENTRY_CB, vp, vp])
     sig("mz_zip_cuda_trim", None, [])
+    sig("mz_zip_cuda_extract_device", i32, [vp, u64, C.c_char_p, vp, u32, C.POINTER(u32), vp, u64, C.POINTER(u64), vp, vp])
+    sig("mz_cuda_zip_parse_directory", i32, [vp, u64, vp, vp])
+    sig("mz_cuda_zip_statuses", i32, [vp, u32, vp, vp, vp])
     return L
 
 
@@ -245,6 +255,36 @@ def crc32_device(tensor, nbytes=None, value=0):
     n = tensor.numel() * tensor.element_size() if nbytes is None else nbytes
     check(lib.mz_cuda_crc32_device(tensor.data_ptr(), n, value, C.byref(out)), "crc32_device")
     return out.value
+
+
+def extract_device(archive, password=None):
+    """Extract every entry of a zip archive held in a CUDA uint8 tensor (mz_zip_cuda_extract_device): the directory is parsed and
+    the entries decoded on the device. Returns (entries, out): entries = [(name, offset, size, crc)] in directory order, the plain
+    bytes of each at out[offset:offset + size] in the CUDA tensor `out`. Raises on any error, as check() does."""
+    import torch
+    lib = load()
+    check(lib.mz_cuda_init(), "mz_cuda_init")
+    assert archive.is_cuda and archive.dtype == torch.uint8, "archive: a CUDA uint8 tensor"
+    archive = archive.contiguous()
+    pw = password.encode() if password is not None else None
+    count, nbytes = C.c_uint32(0), C.c_uint64(0)
+    s = _stream_ptr()
+    n = archive.numel()
+    ptr = archive.data_ptr() if n else None
+    err = lib.mz_zip_cuda_extract_device(ptr, n, pw, None, 0, C.byref(count), None, 0, C.byref(nbytes), None, s)  # sizes only
+    if err not in (MZ_OK, MZ_BUF_ERROR):
+        check(err, "extract_device")
+    table = torch.empty(max(1, count.value) * C.sizeof(ZipDevEntry), dtype=torch.uint8, device=archive.device)
+    out = torch.empty(max(16, nbytes.value), dtype=torch.uint8, device=archive.device)
+    check(lib.mz_zip_cuda_extract_device(ptr, n, pw, table.data_ptr(), count.value, C.byref(count), out.data_ptr(), nbytes.value,
+                                         C.byref(nbytes), None, s), "extract_device")
+    rows = (ZipDevEntry * max(1, count.value)).from_buffer_copy(table.cpu().numpy().tobytes())[:count.value]
+    entries = []
+    if rows:
+        lo = min(r.name_off for r in rows)
+        names = archive[lo:max(r.name_off + r.name_len for r in rows)].cpu().numpy().tobytes()
+        entries = [(names[r.name_off - lo:r.name_off - lo + r.name_len].decode("utf-8", "replace"), r.out_off, r.usize, r.crc) for r in rows]
+    return entries, out[:nbytes.value]
 
 
 def inflate_device(comp, out_cap):

@@ -1,6 +1,7 @@
 /* mz_cuda_api.cu -- the thin extern "C" shim between the C host side and the sm_90a kernels.
  * Declares nothing new: every entry point is documented in include/mz_cuda_batch.h. */
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -18,9 +19,12 @@
 #include "sha256_kernel.cuh"
 #include "wzaes_kernel.cuh"
 #include "zipdir_kernel.cuh"
+#include "zipcd_kernel.cuh"
+#include "../../include/mz_zip_cuda.h"
 
 #define MZ_OK 0
 #define MZ_MEM_ERROR (-4)
+#define MZ_FORMAT_ERROR (-103)
 #define MZ_PARAM_ERROR (-102)
 #define MZ_INTERNAL_ERROR (-104)
 #define MZ_SUPPORT_ERROR (-109)
@@ -32,6 +36,9 @@ static_assert(sizeof(mz_cuda_inflate_state) == sizeof(InflateState), "state layo
 static_assert(sizeof(mz_cuda_spec_summary) == sizeof(SpecSummary), "summary layout");
 static_assert(sizeof(mz_cuda_zip_ent) == sizeof(ZipEnt) && sizeof(mz_cuda_zip_ent) == 64, "zip entry layout");
 static_assert(sizeof(mz_cuda_zip_round) == sizeof(ZipRound), "zip round layout");
+static_assert(sizeof(mz_cuda_zip_dev_entry) == sizeof(ZipDevEnt) && sizeof(mz_cuda_zip_dev_entry) == 72 &&
+                  offsetof(mz_cuda_zip_dev_entry, status) == offsetof(ZipDevEnt, status) && offsetof(ZipDevEnt, status) == 68,
+              "device zip entry layout");
 
 namespace {
 
@@ -496,6 +503,214 @@ int32_t zip_launch(const mz_cuda_zip_round *r, void *stream, int which) {
 int32_t mz_cuda_zip_locate(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 0); }
 int32_t mz_cuda_zip_copy_stored(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 1); }
 int32_t mz_cuda_zip_verify(const mz_cuda_zip_round *r, void *stream) { return zip_launch(r, stream, 2); }
+
+/* ---- K10: the central directory on the device ------------------------------------------------------------------ */
+extern "C++" {
+namespace {
+/* the parse's scratch (19 arrays at most, sized by the summaries read back between stages): freed when the call returns, after
+ * the stream has drained. A fixed table, so nothing can throw through the C entry point. */
+struct ZcScratch {
+    cudaStream_t s;
+    void *p[24];
+    int n = 0;
+    explicit ZcScratch(cudaStream_t st) : s(st) {}
+    ~ZcScratch() {
+        cudaStreamSynchronize(s);
+        for (int i = 0; i < n; i++) cudaFree(p[i]);
+    }
+    template <class T> T *get(uint64_t cnt) {
+        void *q = nullptr;
+        if (n == 24 || cudaMalloc(&q, cnt ? cnt * sizeof(T) : 16) != cudaSuccess) {
+            cudaGetLastError();
+            return nullptr;
+        }
+        p[n++] = q;
+        return (T *)q;
+    }
+};
+
+/* out[i] = in[0] + ... + in[i-1] for i = 0..n */
+template <typename T> int32_t zc_scan(const T *in, uint64_t n, T *out, ZcScratch &w) {
+    const uint64_t nb = n / ZC_TILE + 1;
+    T *part = w.get<T>(nb);
+    if (!part) return MZ_MEM_ERROR;
+    MZ_LAUNCH(zc_scan_reduce_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, w.s, in, n, part);
+    MZ_LAUNCH(zc_scan_parts_kernel<T>, dim3(1), dim3(ZC_THREADS), 0, w.s, part, (uint32_t)nb);
+    MZ_LAUNCH(zc_scan_apply_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, w.s, in, n, (const T *)part, out);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t zc_read_summary(ZcSummary *h, const ZcSummary *d, cudaStream_t s) {
+    CK(cudaMemcpyAsync(h, d, sizeof(*h), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return MZ_OK;
+}
+
+uint32_t zc_grid(uint64_t n) { return (uint32_t)((n + ZC_THREADS - 1) / ZC_THREADS); }
+} // namespace
+} // extern "C++"
+
+int32_t mz_cuda_zip_parse_directory(const void *d_archive, uint64_t len, mz_cuda_zip_dir *dir, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!dir || (!d_archive && len)) return MZ_PARAM_ERROR;
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint8_t *buf = (const uint8_t *)d_archive;
+    dir->err = dir->refuse = MZ_OK;
+    dir->count = dir->njobs = dir->nsha = 0;
+    dir->cd_off = dir->out_bytes = dir->bytes_in = dir->bytes_out = 0;
+    memset(dir->na, 0, sizeof(dir->na));
+    memset(dir->max_clen, 0, sizeof(dir->max_clen));
+    dir->ent = nullptr;
+    dir->sha_expect = nullptr;
+    ZcScratch w(s);
+    ZcSummary h;
+    memset(&h, 0, sizeof(h));
+    h.refuse_idx = 0xffffffffu;
+    ZcSummary *S = w.get<ZcSummary>(1);
+    if (!S) return MZ_MEM_ERROR;
+    CK(cudaMemcpyAsync(S, &h, sizeof(h), cudaMemcpyHostToDevice, s));
+    /* 1. end records */
+    MZ_LAUNCH(zc_end_kernel, dim3(1), dim3(ZC_THREADS), 0, s, buf, len, S);
+    CK(cudaGetLastError());
+    if ((err = zc_read_summary(&h, S, s))) return err;
+    if (h.err) {
+        dir->err = h.err;
+        return MZ_OK;
+    }
+    dir->cd_off = h.cd_off;
+    const uint64_t cd_size = h.cd_size, count = h.count;
+    /* Candidate ranks, the word prefix and the candidate count are 32-bit. Two PK\1\2 signatures cannot overlap (no proper suffix of
+     * the signature is a prefix of it), so candidates lie at least 4 bytes apart and a directory below 16 GiB has fewer than
+     * 2^32 - 2 of them: every rank stays below ZC_BRK. */
+    if (cd_size >= (1ull << 34)) return MZ_SUPPORT_ERROR;
+    const uint8_t *cd = buf + h.cd_off;
+    /* 2. candidates */
+    const uint64_t W = (cd_size + 31) / 32;
+    uint32_t ncand = 0, *bits = nullptr, *wpre = nullptr;
+    if (cd_size) {
+        uint32_t *wcount = w.get<uint32_t>(W);
+        bits = w.get<uint32_t>(W);
+        wpre = w.get<uint32_t>(W + 1);
+        if (!wcount || !bits || !wpre) return MZ_MEM_ERROR;
+        MZ_LAUNCH(zc_cand_kernel, dim3(zc_grid(cd_size)), dim3(ZC_THREADS), 0, s, cd, cd_size, bits, wcount);
+        CK(cudaGetLastError());
+        if ((err = zc_scan(wcount, W, wpre, w))) return err;
+        CK(cudaMemcpyAsync(&ncand, wpre + W, 4, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+    }
+    /* 3. the chain from the first record */
+    const uint32_t slots = (uint32_t)(count < ncand ? count : ncand);
+    uint64_t *rpos = nullptr;
+    if (ncand) {
+        uint64_t *cpos = w.get<uint64_t>(ncand);
+        uint32_t *succ = w.get<uint32_t>(ncand), *ja = w.get<uint32_t>(ncand), *jb = w.get<uint32_t>(ncand), *mark = w.get<uint32_t>(ncand);
+        uint32_t *midx = w.get<uint32_t>((uint64_t)ncand + 1);
+        rpos = w.get<uint64_t>(slots);
+        if (!cpos || !succ || !ja || !jb || !mark || !midx || !rpos) return MZ_MEM_ERROR;
+        MZ_LAUNCH(zc_link_kernel, dim3(zc_grid(cd_size)), dim3(ZC_THREADS), 0, s, cd, cd_size, (const uint32_t *)bits, (const uint32_t *)wpre, cpos, succ,
+                  ja, mark);
+        for (uint32_t k = 0; (1ull << k) < ncand; k++) {
+            MZ_LAUNCH(zc_double_kernel, dim3(zc_grid(ncand)), dim3(ZC_THREADS), 0, s, ncand, mark, (const uint32_t *)ja, jb);
+            std::swap(ja, jb);
+        }
+        CK(cudaGetLastError());
+        if ((err = zc_scan(mark, ncand, midx, w))) return err;
+        MZ_LAUNCH(zc_place_kernel, dim3(zc_grid(ncand)), dim3(ZC_THREADS), 0, s, ncand, (const uint32_t *)mark, (const uint32_t *)midx,
+                  (const uint64_t *)cpos, (const uint32_t *)succ, (uint64_t)slots, rpos, S);
+        CK(cudaGetLastError());
+        if ((err = zc_read_summary(&h, S, s))) return err;
+    }
+    /* where the chain itself ends the list, as the host loop would: a record that does not fit or has no signature, more records
+     * than the end record counts, or fewer */
+    const uint32_t n = (uint32_t)(h.nchain < count ? h.nchain : count);
+    int32_t limit_code = MZ_OK;
+    if (h.nchain == 0 ? cd_size != 0 : (h.nchain > count || h.term == ZC_BRK || h.nchain < count)) limit_code = MZ_FORMAT_ERROR;
+    /* 4. records */
+    ZcRec *rec = nullptr;
+    uint64_t *roff = nullptr;
+    ZcCount *pre = nullptr;
+    if (n) {
+        ZcCount *cnt = w.get<ZcCount>(n);
+        rec = w.get<ZcRec>(n);
+        roff = w.get<uint64_t>(n);
+        pre = w.get<ZcCount>((uint64_t)n + 1);
+        if (!cnt || !rec || !roff || !pre) return MZ_MEM_ERROR;
+        MZ_LAUNCH(zc_records_kernel, dim3(zc_grid(n)), dim3(ZC_THREADS), 0, s, buf, h.cd_off, h.shift, (const uint64_t *)rpos, n, dir->have_password,
+                  dir->password_long, rec, roff, cnt, S);
+        CK(cudaGetLastError());
+        if ((err = zc_scan(cnt, n, pre, w))) return err;
+        MZ_LAUNCH(zc_finish_kernel, dim3(zc_grid(n)), dim3(ZC_THREADS), 0, s, (const ZcRec *)rec, (const uint64_t *)roff, (const ZcCount *)pre, n,
+                  limit_code, S);
+        CK(cudaGetLastError());
+        if ((err = zc_read_summary(&h, S, s))) return err;
+    } else {
+        h.nacc = 0;
+        h.refuse = limit_code;
+    }
+    const uint32_t m = h.nacc;
+    dir->count = m;
+    dir->refuse = h.refuse;
+    dir->out_bytes = h.out;
+    dir->bytes_in = h.cin;
+    dir->bytes_out = h.cout;
+    dir->njobs = h.job;
+    dir->nsha = h.sha;
+    for (int k = 0; k < 4; k++) {
+        dir->na[k] = h.a[k];
+        dir->max_clen[k] = h.max_clen[k];
+    }
+    const bool fits = dir->max_entries >= m && (!dir->decode || dir->out_cap >= h.out); /* otherwise MZ_BUF_ERROR: nothing listed */
+    const bool pub = fits && dir->entries, dec = fits && dir->decode;
+    if (!m || (!pub && !dec)) return MZ_OK;
+    /* 5. extents, tables */
+    const uint64_t *key = roff;
+    if (h.unsorted) {
+        if (m > (1u << 31)) return MZ_SUPPORT_ERROR;
+        uint32_t np = 1;
+        while (np < m) np <<= 1;
+        uint64_t *sorted = w.get<uint64_t>(np);
+        if (!sorted) return MZ_MEM_ERROR;
+        MZ_LAUNCH(zc_pad_kernel, dim3(zc_grid(np)), dim3(ZC_THREADS), 0, s, (const uint64_t *)roff, m, sorted, np);
+        for (uint64_t k = 2; k <= np; k <<= 1)
+            for (uint32_t j = (uint32_t)(k >> 1); j; j >>= 1) MZ_LAUNCH(zc_bitonic_kernel, dim3(zc_grid(np)), dim3(ZC_THREADS), 0, s, sorted, np, (uint32_t)k, j);
+        CK(cudaGetLastError());
+        key = sorted;
+    }
+    ZipEnt *ent = nullptr;
+    uint8_t *sha = nullptr;
+    if (dec) {
+        CK(cudaMalloc(&ent, (size_t)m * sizeof(ZipEnt)));
+        if (cudaMalloc(&sha, (size_t)(h.sha ? h.sha : 1) * 32) != cudaSuccess) {
+            cudaFree(ent);
+            return fail(cudaErrorMemoryAllocation, "cudaMalloc");
+        }
+    }
+    MZ_LAUNCH(zc_fill_kernel, dim3(zc_grid(m)), dim3(ZC_THREADS), 0, s, (const ZcRec *)rec, (const ZcCount *)pre, key, m, h.cd_off, buf,
+              pub ? (ZipDevEnt *)dir->entries : nullptr, ent, sha);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        cudaFree(ent);
+        cudaFree(sha);
+        return fail(e, "zc_fill_kernel");
+    }
+    dir->ent = (mz_cuda_zip_ent *)ent;
+    dir->sha_expect = sha;
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entries, uint32_t *d_first, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (n == 0) return MZ_OK;
+    if (!d_status || !d_entries || !d_first) return MZ_PARAM_ERROR;
+    MZ_LAUNCH(zc_status_kernel, dim3(zc_grid(n)), dim3(ZC_THREADS), 0, (cudaStream_t)stream, d_status, n, (ZipDevEnt *)d_entries, d_first);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
 
 /* workspace carving for K6 (all pieces 256-byte aligned) */
 static inline uint64_t al256(uint64_t v) { return (v + 255) & ~255ull; }

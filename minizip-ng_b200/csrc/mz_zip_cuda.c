@@ -1193,18 +1193,16 @@ static void zr_release(zr_slot *z) {
         zr_free(z);
 }
 
-/* the round's device work; on return h_status and h_out hold the results (z->err: a CUDA error, not an entry's) */
-static void *zr_run(void *arg) {
-    zr_slot *z = (zr_slot *)arg;
-    const double t0 = now_ms();
-    void *s = z->stream;
+/* the round's launches on stream s, from the K9 table in z->d_ent (and digests in z->d_sha) over the stored bytes buf[0, buf_len)
+ * (32 readable bytes past them) into out: locate, K8 per strength (decrypts buf in place), stored copy, K5, K1, K7, verify */
+static int32_t zr_launch(zr_slot *z, uint8_t *buf, uint64_t buf_len, uint8_t *out, void *s) {
     const uint32_t n = z->n;
-    int32_t err = mz_cuda_set_device(z->device);
+    int32_t err = MZ_OK;
     mz_cuda_zip_round R;
     memset(&R, 0, sizeof(R));
-    R.buf = z->d_in;
-    R.buf_len = z->in_used;
-    R.out = z->d_out;
+    R.buf = buf;
+    R.buf_len = buf_len;
+    R.out = out;
     R.ent = z->d_ent;
     R.n = n;
     R.jobs = z->d_job;
@@ -1222,9 +1220,6 @@ static void *zr_run(void *arg) {
     R.keys = z->d_keys;
     R.mac = z->d_mac;
     R.status = z->d_status;
-    if (!err) err = mz_cuda_memcpy_h2d(z->d_in, z->h_in, z->in_used + 32, s); /* K5 reads up to 16 bytes past a stream */
-    if (!err) err = mz_cuda_memcpy_h2d(z->d_ent, z->h_ent, (size_t)n * sizeof(mz_cuda_zip_ent), s);
-    if (!err && z->nsha) err = mz_cuda_memcpy_h2d(z->d_sha, z->h_sha, (size_t)z->nsha * 32, s);
     if (!err) err = mz_cuda_zip_locate(&R, s);
     /* WinZip AES (mz_strm_wzaes.c): keys from password + salt, HMAC of the ciphertext, then the ciphertext becomes the compressed
      * stream in place; one pass per strength present, rows of a strength are contiguous from base */
@@ -1234,9 +1229,9 @@ static void *zr_run(void *arg) {
         const size_t pwl = strlen(z->password);
         err = mz_cuda_memcpy_h2d(z->d_pw, z->password, pwl ? pwl : 1, s);
         if (!err) err = mz_cuda_wzaes_derive(z->d_pw, (uint32_t)pwl, z->d_salt + (size_t)base * 16, z->na[st], st, z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC, s);
-        if (!err) err = mz_cuda_wzaes_hmac(z->d_in, z->d_coff + base, z->d_clen + base, z->na[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC, st,
+        if (!err) err = mz_cuda_wzaes_hmac(buf, z->d_coff + base, z->d_clen + base, z->na[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC, st,
                                            z->d_mac + (size_t)base * 20, s);
-        if (!err) err = mz_cuda_wzaes_ctr(z->d_in, z->d_coff + base, z->d_clen + base, z->na[st], z->max_clen[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC,
+        if (!err) err = mz_cuda_wzaes_ctr(buf, z->d_coff + base, z->d_clen + base, z->na[st], z->max_clen[st], z->d_keys + (size_t)base * MZ_CUDA_WZAES_KEYREC,
                                           st, s);
     }
     if (!err) err = mz_cuda_zip_copy_stored(&R, s);
@@ -1244,9 +1239,23 @@ static void *zr_run(void *arg) {
         err = mz_cuda_memset(z->d_state, 0, (size_t)z->njobs * sizeof(mz_cuda_inflate_state), s);
         if (!err) err = mz_cuda_inflate_streams(z->d_job, z->d_state, z->njobs, s);
     }
-    if (!err) err = mz_cuda_crc32_segments(z->d_out, 0, 0, z->d_seg_off, z->d_seg_len, n, z->d_residue, z->d_crc, s);
-    if (!err && z->nsha) err = mz_cuda_sha256_batch(z->d_out, z->d_seg_off, z->d_seg_len64, n, z->d_digest, s);
+    if (!err) err = mz_cuda_crc32_segments(out, 0, 0, z->d_seg_off, z->d_seg_len, n, z->d_residue, z->d_crc, s);
+    if (!err && z->nsha) err = mz_cuda_sha256_batch(out, z->d_seg_off, z->d_seg_len64, n, z->d_digest, s);
     if (!err) err = mz_cuda_zip_verify(&R, s);
+    return err;
+}
+
+/* the round's device work; on return h_status and h_out hold the results (z->err: a CUDA error, not an entry's) */
+static void *zr_run(void *arg) {
+    zr_slot *z = (zr_slot *)arg;
+    const double t0 = now_ms();
+    void *s = z->stream;
+    const uint32_t n = z->n;
+    int32_t err = mz_cuda_set_device(z->device);
+    if (!err) err = mz_cuda_memcpy_h2d(z->d_in, z->h_in, z->in_used + 32, s); /* K5 reads up to 16 bytes past a stream */
+    if (!err) err = mz_cuda_memcpy_h2d(z->d_ent, z->h_ent, (size_t)n * sizeof(mz_cuda_zip_ent), s);
+    if (!err && z->nsha) err = mz_cuda_memcpy_h2d(z->d_sha, z->h_sha, (size_t)z->nsha * 32, s);
+    if (!err) err = zr_launch(z, z->d_in, z->in_used, z->d_out, s);
     if (!err) err = mz_cuda_memcpy_d2h(z->h_status, z->d_status, (size_t)n * 4, s);
     if (!err) err = mz_cuda_memcpy_d2h(z->h_out, z->d_out, z->out_used, s);
     if (!err) err = mz_cuda_stream_sync(s);
@@ -1953,6 +1962,135 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
     free(rfirst);
     free(ent);
     free(names);
+    if (stats)
+        *stats = st;
+    return err;
+}
+
+/* ---- an archive in device memory (mz_zip_cuda_extract_device) ------------------------------------------------------------ */
+/* the round arrays K9 / K8 / K5 / K1 / K7 need for n entries, and the first-failure word, carved from one device allocation (returned;
+ * NULL when it fails). The K9 table and the digests come from the directory parse. */
+static uint8_t *zd_carve(zr_slot *z, uint32_t n, uint32_t **first) {
+    const size_t m = n ? n : 1;
+    const size_t sz[17] = {m * 4, m * sizeof(mz_cuda_inflate_job), m * sizeof(mz_cuda_inflate_state), m * 8, m * 8, m * 8, m * 8, m * 8, m * 4,
+                           m * 4, m * 4, z->nsha ? m * 32 : 32, m * 16, m * MZ_CUDA_WZAES_KEYREC, 256, m * 20, 4};
+    size_t off[17], total = 0;
+    for (int k = 0; k < 17; k++) {
+        off[k] = total;
+        total += (sz[k] + 255) & ~(size_t)255;
+    }
+    uint8_t *w = (uint8_t *)mz_cuda_malloc(total);
+    if (!w)
+        return NULL;
+    z->d_status = (uint32_t *)(w + off[0]);
+    z->d_job = (mz_cuda_inflate_job *)(w + off[1]);
+    z->d_state = (mz_cuda_inflate_state *)(w + off[2]);
+    z->d_seg_off = (uint64_t *)(w + off[3]);
+    z->d_seg_len64 = (uint64_t *)(w + off[4]);
+    z->d_data_off = (uint64_t *)(w + off[5]);
+    z->d_coff = (uint64_t *)(w + off[6]);
+    z->d_clen = (uint64_t *)(w + off[7]);
+    z->d_seg_len = (uint32_t *)(w + off[8]);
+    z->d_residue = (uint32_t *)(w + off[9]);
+    z->d_crc = (uint32_t *)(w + off[10]);
+    z->d_digest = w + off[11];
+    z->d_salt = w + off[12];
+    z->d_keys = w + off[13];
+    z->d_pw = w + off[14];
+    z->d_mac = w + off[15];
+    *first = (uint32_t *)(w + off[16]);
+    return w;
+}
+
+int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
+                                   uint32_t *count, void *d_out, uint64_t out_cap, uint64_t *out_bytes, mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    if (!count || !out_bytes || (!d_archive && len) || ((uintptr_t)d_out & 15) || (!d_entries && max_entries))
+        return MZ_PARAM_ERROR;
+    *count = 0;
+    *out_bytes = 0;
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    const double t0 = now_ms();
+    mz_cuda_zip_dir dir;
+    memset(&dir, 0, sizeof(dir));
+    dir.have_password = password != NULL;
+    dir.password_long = password && strlen(password) > 128;
+    dir.entries = d_entries;
+    dir.max_entries = max_entries;
+    dir.decode = d_out != NULL;
+    dir.out_cap = out_cap;
+    int32_t err = mz_cuda_zip_parse_directory(d_archive, len, &dir, stream);
+    if (err == MZ_OK && dir.err)
+        err = dir.err; /* the archive as a whole */
+    st.pack_ms = now_ms() - t0;
+    if (err) {
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    *count = dir.count;
+    *out_bytes = dir.out_bytes;
+    st.entries = dir.count;
+    st.bytes_in = dir.bytes_in;
+    st.bytes_out = dir.bytes_out;
+    if (max_entries < dir.count || (d_out && out_cap < dir.out_bytes))
+        err = MZ_BUF_ERROR;
+    else if (!d_out || !dir.count)
+        err = dir.refuse;
+    else {
+        zr_slot z;
+        memset(&z, 0, sizeof(z));
+        z.n = dir.count;
+        z.njobs = dir.njobs;
+        z.nsha = dir.nsha;
+        memcpy(z.na, dir.na, sizeof(z.na));
+        memcpy(z.max_clen, dir.max_clen, sizeof(z.max_clen));
+        z.password = password;
+        z.d_ent = dir.ent;
+        z.d_sha = (uint8_t *)dir.sha_expect;
+        const double t1 = now_ms();
+        /* K8 decrypts in place: AES entries are decoded from a copy of the bytes in front of the directory */
+        const int aes = dir.na[1] || dir.na[2] || dir.na[3];
+        uint8_t *buf = (uint8_t *)d_archive, *copy = NULL;
+        uint32_t *d_first = NULL;
+        uint8_t *work = zd_carve(&z, dir.count, &d_first);
+        if (!work || (aes && !(copy = (uint8_t *)mz_cuda_malloc(dir.cd_off + 32))))
+            err = MZ_MEM_ERROR;
+        st.setup_ms = now_ms() - t1;
+        const double t2 = now_ms();
+        if (!err && copy) {
+            err = mz_cuda_memcpy_d2d(copy, d_archive, dir.cd_off, stream);
+            if (!err) err = mz_cuda_memset(copy + dir.cd_off, 0, 32, stream);
+            buf = copy;
+        }
+        /* buf_len = cd_off: every stream ends at or before the directory, and behind cd_off lie at least one 46-byte directory
+         * record and the 22-byte end record, so K5's 16-byte over-read and the stored copy's word reads stay inside [0, len) */
+        if (!err) err = zr_launch(&z, buf, dir.cd_off, (uint8_t *)d_out, stream);
+        if (!err) err = mz_cuda_memset(d_first, 0xff, 4, stream);
+        if (!err) err = mz_cuda_zip_statuses(z.d_status, z.n, d_entries, d_first, stream);
+        uint32_t first = 0xffffffffu, word = 0;
+        if (!err) err = mz_cuda_memcpy_d2h(&first, d_first, 4, stream);
+        if (!err) err = mz_cuda_stream_sync(stream);
+        if (!err && first < z.n) {
+            err = mz_cuda_memcpy_d2h(&word, z.d_status + first, 4, stream);
+            if (!err) err = mz_cuda_stream_sync(stream);
+            if (!err) err = -(int32_t)(word & 0xffffu);
+        }
+        if (!err) err = dir.refuse;
+        st.gpu_ms = now_ms() - t2;
+        st.rounds = 1;
+        mz_cuda_stream_sync(stream);
+        mz_cuda_free(copy);
+        mz_cuda_free(work);
+    }
+    mz_cuda_free(dir.ent);
+    mz_cuda_free(dir.sha_expect);
     if (stats)
         *stats = st;
     return err;
