@@ -11,6 +11,12 @@
 #ifdef MZ_EMU
 #include "cuda_emu.h"
 #define MZ_DYN_SMEM(name) uint8_t *name = emu_dyn_smem
+/* The emulator's preemption and race-check hooks (tests/emu/cuda_emu.h defines them). Without them every access below is a plain
+ * load or store. */
+#ifndef MZ_EMU_ACCESS
+#define MZ_EMU_ACCESS(p, bytes, kind, newval)
+#define MZ_EMU_PREEMPT()
+#endif
 #else
 #include <cuda_runtime.h>
 #define MZ_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
@@ -34,6 +40,7 @@ __device__ __forceinline__ uint32_t load32u(const uint8_t *base, uint32_t p) {
 /* streaming 128-bit global load that does not pollute L1 */
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
 #ifdef MZ_EMU
+    MZ_EMU_PREEMPT();
     return *p;
 #else
     uint4 r;
@@ -49,22 +56,40 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
  * emulator the "address" is a byte offset into the emulated dynamic shared memory. */
 struct Smem {
 #ifdef MZ_EMU
+    /* every access first passes MZ_EMU_ACCESS: a seeded preemption point and the shared-memory race check (cuda_emu.h) */
     uint8_t *b;
     __device__ __forceinline__ void init(uint8_t *base) { b = base; }
-    __device__ __forceinline__ uint32_t ld32(uint32_t off) const { return *(const uint32_t *)(b + (int32_t)off); }
-    __device__ __forceinline__ uint32_t ld16(uint32_t off) const { return *(const uint16_t *)(b + (int32_t)off); }
-    __device__ __forceinline__ uint32_t ld8(uint32_t off) const { return b[(int32_t)off]; }
-    __device__ __forceinline__ void st32(uint32_t off, uint32_t v) const { *(uint32_t *)(b + (int32_t)off) = v; }
-    __device__ __forceinline__ void st16(uint32_t off, uint32_t v) const { *(uint16_t *)(b + (int32_t)off) = (uint16_t)v; }
-    __device__ __forceinline__ void red_or32(uint32_t off, uint32_t v) const { *(uint32_t *)(b + (int32_t)off) |= v; }
-    __device__ __forceinline__ void red_add32(uint32_t off, uint32_t v) const { *(uint32_t *)(b + (int32_t)off) += v; }
-    __device__ __forceinline__ void red_min32(uint32_t off, uint32_t v) const { uint32_t *p = (uint32_t *)(b + (int32_t)off); if (v < *p) *p = v; }
-    __device__ __forceinline__ void st16_if(bool p, uint32_t off, uint32_t v) const { if (p) st16(off, v); }
-    __device__ __forceinline__ void red_add32_if(bool p, uint32_t off, uint32_t v) const { if (p) red_add32(off, v); }
-    __device__ __forceinline__ void red_or32_if(bool p, uint32_t off, uint32_t v) const { if (p) red_or32(off, v); }
-    __device__ __forceinline__ uint2 ld64(uint32_t off) const { return *(const uint2 *)(b + (int32_t)off); }
-    __device__ __forceinline__ void st64(uint32_t off, uint32_t x, uint32_t y) const { *(uint2 *)(b + (int32_t)off) = make_uint2(x, y); }
-    __device__ __forceinline__ void st128(uint32_t off, uint32_t x, uint32_t y, uint32_t z, uint32_t w) const { *(uint4 *)(b + (int32_t)off) = make_uint4(x, y, z, w); }
+    __device__ __forceinline__ uint8_t *p(uint32_t off) const { return b + (int32_t)off; }
+    __device__ __forceinline__ uint32_t ld32(uint32_t off) const { MZ_EMU_ACCESS(p(off), 4, EMU_ACC_READ, nullptr); return *(const uint32_t *)p(off); }
+    __device__ __forceinline__ uint32_t ld16(uint32_t off) const { MZ_EMU_ACCESS(p(off), 2, EMU_ACC_READ, nullptr); return *(const uint16_t *)p(off); }
+    __device__ __forceinline__ uint32_t ld8(uint32_t off) const { MZ_EMU_ACCESS(p(off), 1, EMU_ACC_READ, nullptr); return *p(off); }
+    __device__ __forceinline__ void st32(uint32_t off, uint32_t v) const { MZ_EMU_ACCESS(p(off), 4, EMU_ACC_WRITE, &v); *(uint32_t *)p(off) = v; }
+    __device__ __forceinline__ void st16(uint32_t off, uint32_t v) const {
+        const uint16_t h = (uint16_t)v;
+        MZ_EMU_ACCESS(p(off), 2, EMU_ACC_WRITE, &h);
+        *(uint16_t *)p(off) = h;
+    }
+    __device__ __forceinline__ void red_or32(uint32_t off, uint32_t v) const { MZ_EMU_ACCESS(p(off), 4, EMU_ACC_ATOMIC, nullptr); *(uint32_t *)p(off) |= v; }
+    __device__ __forceinline__ void red_add32(uint32_t off, uint32_t v) const { MZ_EMU_ACCESS(p(off), 4, EMU_ACC_ATOMIC, nullptr); *(uint32_t *)p(off) += v; }
+    __device__ __forceinline__ void red_min32(uint32_t off, uint32_t v) const {
+        MZ_EMU_ACCESS(p(off), 4, EMU_ACC_ATOMIC, nullptr);
+        uint32_t *q = (uint32_t *)p(off);
+        if (v < *q) *q = v;
+    }
+    __device__ __forceinline__ void st16_if(bool c, uint32_t off, uint32_t v) const { if (c) st16(off, v); }
+    __device__ __forceinline__ void red_add32_if(bool c, uint32_t off, uint32_t v) const { if (c) red_add32(off, v); }
+    __device__ __forceinline__ void red_or32_if(bool c, uint32_t off, uint32_t v) const { if (c) red_or32(off, v); }
+    __device__ __forceinline__ uint2 ld64(uint32_t off) const { MZ_EMU_ACCESS(p(off), 8, EMU_ACC_READ, nullptr); return *(const uint2 *)p(off); }
+    __device__ __forceinline__ void st64(uint32_t off, uint32_t x, uint32_t y) const {
+        const uint2 v = make_uint2(x, y);
+        MZ_EMU_ACCESS(p(off), 8, EMU_ACC_WRITE, &v);
+        *(uint2 *)p(off) = v;
+    }
+    __device__ __forceinline__ void st128(uint32_t off, uint32_t x, uint32_t y, uint32_t z, uint32_t w) const {
+        const uint4 v = make_uint4(x, y, z, w);
+        MZ_EMU_ACCESS(p(off), 16, EMU_ACC_WRITE, &v);
+        *(uint4 *)p(off) = v;
+    }
     /* absolute forms: addr() folds the window base into a region base once, the *_a accessors then take that address as it is */
     __device__ __forceinline__ uint32_t addr(uint32_t off) const { return off; }
     __device__ __forceinline__ uint32_t ld32_a(uint32_t a) const { return ld32(a); }

@@ -7,8 +7,31 @@
  * the device for race-free code. It is never linked into the product library and never used as a
  * fallback: the product .so is built by nvcc only and fails loudly without a GPU.
  *
- * Not modelled: real concurrency/races, memory-ordering, bank conflicts, timing, TMA/mbarrier (kernels
+ * Not modelled: real concurrency, memory-ordering, bank conflicts, timing, TMA/mbarrier (kernels
  * guard their PTX with #ifndef MZ_EMU and use a plain copy under emulation).
+ *
+ * Seeded schedules (MZ_EMU_SCHED=<seed>, unset or 0 = the fixed schedule: tid order, blockIdx order, 0xCD fill):
+ *  - every scheduler pass runs the runnable fibers of a CTA in a fresh seeded permutation;
+ *  - before every Smem accessor, emulated atomic and ldg_stream a fiber yields with a small seeded probability
+ *    (EMU_PREEMPT_ONE_IN), so lanes of one warp interleave between two shared accesses as they can on Volta and later;
+ *  - each launch visits its CTAs in a seeded permutation of blockIdx;
+ *  - at every CTA, dynamic shared memory and all static __shared__ storage (the mz_emu_shared section) are filled
+ *    with seeded random bytes, so a read of shared memory nobody wrote gives seed-dependent output.
+ *
+ * Shared-memory race checker (MZ_EMU_RACE=1; most useful together with a seed):
+ *  - shadow state per 4-byte word of the CTA's dynamic shared memory and of the static __shared__ storage records the
+ *    last write (thread, plain or atomic, byte mask) and up to EMU_RACE_READERS reads since it;
+ *  - happens-before comes only from a block barrier, from a named barrier in which both threads' whole warps took
+ *    part, and from a warp barrier or warp collective of one warp whose mask holds both lanes (all transitively);
+ *  - reported: a plain write followed by a read or a write of an overlapping byte by another thread, and a read
+ *    followed by a write (plain or atomic) by another thread, with no such edge between them. Atomic against
+ *    atomic is never reported, and neither is an atomic followed by a plain read. A plain write that leaves the
+ *    bytes as they are (several threads storing the same value, an idiom the kernels use) is allowed;
+ *  - the report names the launch, the block, the word and both threads, then aborts;
+ *  - coverage: only the Smem accessors (mzcuda_common.cuh) and the emulated atomics are seen. Shared memory read or
+ *    written through raw pointers or array indexing (staging through uint8_t pointers, static __shared__ arrays,
+ *    inflate's table structs) is invisible to it; poisoning still covers those. When more than EMU_RACE_READERS
+ *    threads read a word concurrently, only that many reads are kept for the check against the next write.
  */
 #ifndef CUDA_EMU_H
 #define CUDA_EMU_H
@@ -33,7 +56,9 @@
 #define __restrict__
 #define __launch_bounds__(...)
 #define __align__(n) __attribute__((aligned(n)))
-#define __shared__ static
+/* static __shared__ variables live in one section so that the scheduler can poison them at every CTA and the race checker can
+ * map their addresses (cuda_emu.cc, __start_/__stop_mz_emu_shared) */
+#define __shared__ static __attribute__((section("mz_emu_shared")))
 #define __constant__ static
 
 struct emu_dim3 {
@@ -65,8 +90,9 @@ void emu_run_block(unsigned nthreads, void (*entry)(void *), void *arg, size_t d
 
 struct emu_warp_state {
     uint64_t slot[32];
-    int arrived;
-    unsigned gen;
+    unsigned arrived;   /* lanes waiting at a warp barrier */
+    unsigned want[32];  /* the mask each waiting lane named (its own bit included) */
+    unsigned gen[32];   /* per lane: bumped when its warp barrier releases it */
     unsigned live_mask; /* lanes that exist and have not exited */
 };
 extern emu_warp_state *emu_cur_warp(void);
@@ -74,6 +100,24 @@ extern int emu_lane(void);
 void emu_block_barrier(void);
 void emu_named_barrier(int id, int nthreads);
 void emu_warp_barrier(unsigned mask);
+
+/* seeded schedules and the race checker (cuda_emu.cc) */
+extern int emu_sched_on, emu_race_on, emu_hooks_on; /* emu_hooks_on = either: one test on the hot path when both are off */
+void emu_preempt_slow(void);
+static inline void emu_preempt(void) {
+    if (emu_sched_on) emu_preempt_slow();
+}
+enum { EMU_ACC_READ = 0, EMU_ACC_WRITE = 1, EMU_ACC_ATOMIC = 2 };
+void emu_access_slow(const void *p, unsigned bytes, int kind, const void *newval);
+/* one shared-memory access through an Smem accessor or an atomic: a possible preemption point, then the race check. newval is
+ * the bytes a plain write is about to store. */
+static inline void emu_access(const void *p, unsigned bytes, int kind, const void *newval = nullptr) {
+    if (__builtin_expect(emu_hooks_on, 0)) emu_access_slow(p, bytes, kind, newval);
+}
+
+/* the hooks as the Smem accessors and ldg_stream call them (mzcuda_common.cuh) */
+#define MZ_EMU_ACCESS(p, bytes, kind, newval) emu_access((p), (bytes), (kind), (newval))
+#define MZ_EMU_PREEMPT() emu_preempt()
 
 static inline void __syncthreads() { emu_block_barrier(); }
 static inline void __syncwarp(unsigned mask = 0xffffffffu) { emu_warp_barrier(mask); }
@@ -239,13 +283,14 @@ static inline unsigned __byte_perm(unsigned a, unsigned b, unsigned s) {
 static inline unsigned __umulhi(unsigned a, unsigned b) { return (unsigned)(((uint64_t)a * b) >> 32); }
 template <typename T> static inline T __ldg(const T *p) { return *p; }
 
-template <typename T> static inline T atomicAdd(T *p, T v) { T o = *p; *p = o + v; return o; }
-template <typename T> static inline T atomicOr(T *p, T v) { T o = *p; *p = o | v; return o; }
-template <typename T> static inline T atomicXor(T *p, T v) { T o = *p; *p = o ^ v; return o; }
-template <typename T> static inline T atomicMax(T *p, T v) { T o = *p; if (v > o) *p = v; return o; }
-template <typename T> static inline T atomicMin(T *p, T v) { T o = *p; if (v < o) *p = v; return o; }
-template <typename T> static inline T atomicExch(T *p, T v) { T o = *p; *p = v; return o; }
-template <typename T> static inline T atomicCAS(T *p, T c, T v) { T o = *p; if (o == c) *p = v; return o; }
+/* an emulated atomic is a plain read-modify-write that no other fiber can split: the preemption point comes before it */
+template <typename T> static inline T atomicAdd(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; *p = o + v; return o; }
+template <typename T> static inline T atomicOr(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; *p = o | v; return o; }
+template <typename T> static inline T atomicXor(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; *p = o ^ v; return o; }
+template <typename T> static inline T atomicMax(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; if (v > o) *p = v; return o; }
+template <typename T> static inline T atomicMin(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; if (v < o) *p = v; return o; }
+template <typename T> static inline T atomicExch(T *p, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; *p = v; return o; }
+template <typename T> static inline T atomicCAS(T *p, T c, T v) { emu_access(p, sizeof(T), EMU_ACC_ATOMIC); T o = *p; if (o == c) *p = v; return o; }
 
 /* ---- launch ---------------------------------------------------------------------------------- */
 template <typename F> struct emu_thunk {
@@ -257,16 +302,16 @@ template <typename F> struct emu_thunk {
  * launches from several host threads (the zip writer's round workers) */
 void emu_launch_lock(void);
 void emu_launch_unlock(void);
+/* the order in which a launch visits its CTAs (linear block indices): 0..n-1, or a seeded permutation of it */
+const std::vector<uint64_t> &emu_block_order(uint64_t nblocks);
 template <typename F> static inline void emu_launch(dim3 grid, dim3 block, size_t smem, F body) {
     emu_launch_lock();
     gridDim = grid;
     blockDim = block;
-    for (unsigned bz = 0; bz < grid.z; bz++)
-        for (unsigned by = 0; by < grid.y; by++)
-            for (unsigned bx = 0; bx < grid.x; bx++) {
-                blockIdx = emu_dim3(bx, by, bz);
-                emu_run_block(block.x * block.y * block.z, &emu_thunk<F>::call, &body, smem);
-            }
+    for (uint64_t b : emu_block_order((uint64_t)grid.x * grid.y * grid.z)) {
+        blockIdx = emu_dim3((unsigned)(b % grid.x), (unsigned)(b / grid.x % grid.y), (unsigned)(b / grid.x / grid.y));
+        emu_run_block(block.x * block.y * block.z, &emu_thunk<F>::call, &body, smem);
+    }
     emu_launch_unlock();
 }
 /* MZ_LAUNCH(kernel, grid, block, smem, stream, args...) */
