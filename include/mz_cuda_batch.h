@@ -241,6 +241,50 @@ int32_t mz_cuda_zip_parse_directory(const void *d_archive, uint64_t len, mz_cuda
  * index of the first failing entry (the caller sets it to 0xffffffff first) */
 int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entries, uint32_t *d_first, void *stream);
 
+/* ---- K11: a zip archive written into device memory (csrc/zipwr_kernel.cuh) --------------------------------------------
+ * The device half of mz_zip_cuda_write_device (include/mz_zip_cuda.h). One call state, device pointers unless noted; the host
+ * carves the arrays and runs: items (validation, per-item counts and their exclusive scan pre[0..n]), chunks (the K2+K3 / K1
+ * chunk table and K7's segments), per round K2+K3 + K1 over chunks [c0, c0 + m) then place (stream offsets S, destinations dst,
+ * copy lengths glen: 0 for a chunk that would pass cap) then K4 mz_cuda_gather(slots, stride, glen + c0, m, dst + c0, archive),
+ * entries (CRC fold, sizes, local-header offsets, directory record sizes and their scan e_cdpre[0..n]), [K8 over e_coff /
+ * e_csize], emit (local headers, salts, verifiers, authentication codes, directory, end records, the mz_cuda_zip_dev_entry
+ * table). `part`: scan scratch of (max(n, m) / MZ_CUDA_ZIP_WR_TILE + 1) x 48 bytes. A round holds at most 32768 chunks. */
+#define MZ_CUDA_ZIP_WR_TILE 2048u
+typedef struct mz_cuda_zip_wr_count { /* per item; pre[e] = the sum over the items in front of e */
+    uint64_t chunks;    /* 64 KiB chunks (an empty entry has one) */
+    uint64_t overhead;  /* local header + name + extra fields + salt + verifier + authentication code */
+    uint64_t bytes;     /* plain bytes */
+    uint64_t out16;     /* plain bytes rounded up to 16 (mz_zip_cuda_extract_device's output layout) */
+    uint64_t bound;     /* mz_cuda_deflate_slot_bound of every chunk */
+    uint64_t cd;        /* directory record without a zip64 field */
+} mz_cuda_zip_wr_count;
+typedef struct mz_cuda_zip_wr {
+    const void *data, *names;
+    const void *items;                     /* mz_cuda_zip_dev_item[n] */
+    uint32_t n, aes, sha, dos_now;         /* aes: WinZip AES strength or 0; sha: hash fields; dos_now: the date of items with 0 */
+    void *archive;
+    uint64_t cap;
+    uint64_t *bad;                         /* 1 word, ~0 before items: index << 1 | (0 = MZ_PARAM_ERROR, 1 = MZ_SUPPORT_ERROR) */
+    mz_cuda_zip_wr_count *cnt, *pre;       /* n, n + 1 */
+    void *part;
+    uint64_t nch;                          /* host: pre[n].chunks */
+    uint64_t *c_off;                       /* per chunk (nch) ... */
+    uint32_t *c_len;
+    uint8_t *c_flags;
+    uint32_t *c_item, *out_len, *residue, *glen;
+    uint64_t *S, *dst;                     /* S: nch + 1, S[0] = 0 */
+    uint64_t *e_lh, *e_csize, *e_cd, *e_cdpre, *e_coff, *e_off, *e_len; /* per entry (e_cdpre: n + 1) */
+    uint32_t *e_crc;
+    uint64_t *max_csize;                   /* 1 word, 0 before entries */
+    const void *digest, *salt, *keys, *mac; /* per entry: SHA-256 (sha), K8 salt / key record / HMAC (aes) */
+    void *entries;                         /* mz_cuda_zip_dev_entry[n] or NULL */
+} mz_cuda_zip_wr;
+int32_t mz_cuda_zip_wr_items(const mz_cuda_zip_wr *w, uint32_t data_null, uint32_t names_null, void *stream);
+int32_t mz_cuda_zip_wr_chunks(const mz_cuda_zip_wr *w, void *stream);
+int32_t mz_cuda_zip_wr_place(const mz_cuda_zip_wr *w, uint64_t c0, uint32_t m, void *stream);
+int32_t mz_cuda_zip_wr_entries(const mz_cuda_zip_wr *w, void *stream);
+int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t cd_size, void *stream);
+
 /* ---- K6: one long foreign stream, segment-speculative (csrc/inflate_spec_kernel.cuh) ------------------------
  * One ROUND decodes as much of the compressed window d_in[0..in_avail) as can be proven, starting at the block
  * boundary `start_bit` (absolute bit; the serial decoder's state must be at a block header), into

@@ -167,6 +167,41 @@ typedef struct mz_cuda_zip_dev_entry {
 int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
                                    uint32_t *count, void *d_out, uint64_t out_cap, uint64_t *out_bytes, mz_cuda_zip_stats *stats, void *stream);
 
+/* ---- an archive written into device memory from entries in device memory ---------------------------------------------
+ * The archive mz_zip_cuda_write_archive (flags with MZ_ZIP_CUDA_AES: mz_zip_cuda_write_archive_aes) writes for the same entries,
+ * level, flags and dates, byte for byte (with AES only the random salts and what follows from them differ), built in device memory
+ * from entries in device memory: d_items[count] (device), each naming its plain bytes at d_data + data_off and its name at d_names +
+ * name_off. Validation, layout, local headers, CRC-32, the central directory and the end records are done on the device (K11 with
+ * K2+K3, K1, K4, K7, K8); only scalars cross PCIe, and with AES the per-entry salts (from getrandom). Synchronous on `stream`.
+ *   - flags: MZ_ZIP_CUDA_HASH_SHA256 and MZ_ZIP_CUDA_AES only (MZ_ZIP_CUDA_ALL_DEVICES: MZ_PARAM_ERROR); level 0..9 or -1 (= 6);
+ *     password and aes_strength as for mz_zip_cuda_write_archive_aes, password ignored without MZ_ZIP_CUDA_AES.
+ *   - errors: argument errors first, in the host writer's order; then the first invalid item in index order: MZ_PARAM_ERROR for its
+ *     name (length 0 or above 65535, a NUL byte) or pointers (d_names NULL, d_data NULL with size > 0), MZ_SUPPORT_ERROR for a size
+ *     of 0xffff0000 or more. Nothing is compressed or written then.
+ *   - an entry just below 4 GiB whose stored size (compressed stream, with AES plus salt, verifier and authentication code) reaches
+ *     0xffffffff cannot be described by its local header: MZ_INTERNAL_ERROR after compression, as mz_zip_cuda_write_archive returns.
+ *   - d_archive == NULL: sizing call, MZ_OK with *archive_len = an upper bound of the archive's length; nothing is compressed.
+ *   - cap smaller than the archive: MZ_BUF_ERROR with *archive_len = the exact length; bytes below cap may have been written.
+ *     No byte at or beyond cap is ever written. On success *archive_len = the exact length.
+ *   - d_data, d_names and d_items are only read; AES encrypts inside d_archive.
+ *   - d_entries (optional, device): one mz_cuda_zip_dev_entry per item, the row mz_zip_cuda_extract_device lists for the archive.
+ *   - chunks are compressed in rounds of MZ_CUDA_ZIP_ROUND_MB MiB of plain bytes (default 1024), so scratch is bounded; every call
+ *     allocates its own.
+ *   - stats: entries, bytes_in, bytes_out as the host writer counts them, rounds, pack_ms = validation and planning, gpu_ms =
+ *     compression to the last kernel, setup_ms = scratch allocation. */
+typedef struct mz_cuda_zip_dev_item {
+    uint64_t data_off;    /* the entry's plain bytes at d_data + data_off (any alignment; items may share bytes) */
+    uint64_t size;        /* below 0xffff0000, as mz_zip_cuda_write_archive */
+    uint64_t name_off;    /* name at d_names + name_off: name_len bytes, no terminator */
+    uint32_t name_len;    /* 1..65535, no NUL byte inside */
+    uint32_t dos_date;    /* MS-DOS date/time exactly as the headers store it; 0 = the time of the call */
+    uint32_t external_fa; /* 0 = regular file 0644, as mz_cuda_zip_item */
+    uint32_t reserved;    /* 0 */
+} mz_cuda_zip_dev_item;   /* 40 bytes */
+int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags,
+                                 const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
+                                 mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream);
+
 /* sizeof the mz_zip_file mirror this library was built with: the host asserts it equals sizeof(mz_zip_file) */
 uint32_t mz_zip_cuda_abi_file_info_size(void);
 

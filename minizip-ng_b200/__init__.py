@@ -58,9 +58,11 @@ EXPORTS = [
     "mz_cuda_stream_wait_event", "mz_cuda_gather", "mz_cuda_scatter_blobs",
     # include/mz_zip_cuda.h
     "mz_zip_cuda_add_buffers", "mz_zip_cuda_add_buffers_ex", "mz_zip_cuda_write_archive", "mz_zip_cuda_trim", "mz_zip_cuda_write_archive_aes", "mz_zip_cuda_extract_all",
-    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_extract_device", "mz_zip_cuda_abi_file_info_size",
+    "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_extract_device", "mz_zip_cuda_write_device", "mz_zip_cuda_abi_file_info_size",
     # include/mz_cuda_batch.h, K9 and K10
     "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify", "mz_cuda_zip_parse_directory", "mz_cuda_zip_statuses",
+    # include/mz_cuda_batch.h, K11
+    "mz_cuda_zip_wr_items", "mz_cuda_zip_wr_chunks", "mz_cuda_zip_wr_place", "mz_cuda_zip_wr_entries", "mz_cuda_zip_wr_emit",
 ]
 
 # mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
@@ -85,6 +87,20 @@ class ZipItem(C.Structure):
     """mz_cuda_zip_item (include/mz_zip_cuda.h)"""
     _fields_ = [("filename", C.c_char_p), ("data", C.c_void_p), ("size", C.c_int64), ("modified_date", C.c_int64),
                 ("external_fa", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class ZipDevItem(C.Structure):
+    """mz_cuda_zip_dev_item (include/mz_zip_cuda.h)"""
+    _fields_ = [("data_off", C.c_uint64), ("size", C.c_uint64), ("name_off", C.c_uint64), ("name_len", C.c_uint32), ("dos_date", C.c_uint32),
+                ("external_fa", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+def dos_date(t):
+    """the MS-DOS date/time the zip headers store for unix time t, in local time (the native writer's za_dos_date)"""
+    import time
+    tm = time.localtime(t)
+    year = tm.tm_year - 1980 if tm.tm_year >= 1980 else 0
+    return ((tm.tm_mday + 32 * tm.tm_mon + 512 * year) << 16) | (tm.tm_sec // 2 + 32 * tm.tm_min + 2048 * tm.tm_hour)
 
 
 def load():
@@ -174,6 +190,7 @@ def configure(L):
     sig("mz_zip_cuda_extract_archive", i32, [vp, C.c_char_p, u32, ZIP_ENTRY_CB, vp, vp])
     sig("mz_zip_cuda_trim", None, [])
     sig("mz_zip_cuda_extract_device", i32, [vp, u64, C.c_char_p, vp, u32, C.POINTER(u32), vp, u64, C.POINTER(u64), vp, vp])
+    sig("mz_zip_cuda_write_device", i32, [vp, vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp, u64, C.POINTER(u64), vp, vp, vp])
     sig("mz_cuda_zip_parse_directory", i32, [vp, u64, vp, vp])
     sig("mz_cuda_zip_statuses", i32, [vp, u32, vp, vp, vp])
     return L
@@ -285,6 +302,43 @@ def extract_device(archive, password=None):
         names = archive[lo:max(r.name_off + r.name_len for r in rows)].cpu().numpy().tobytes()
         entries = [(names[r.name_off - lo:r.name_off - lo + r.name_len].decode("utf-8", "replace"), r.out_off, r.usize, r.crc) for r in rows]
     return entries, out[:nbytes.value]
+
+
+def write_device(files, level=6, sha256=False, password=None, aes_strength=3, mtime=None):
+    """Write a zip archive into device memory from entries in device memory (mz_zip_cuda_write_device): files = [(name, CUDA uint8
+    tensor)], all on the current device; the tensors may be separate allocations. The archive is what write_archive writes for the same
+    bytes (with a password: WinZip AES of aes_strength). mtime: unix time of every entry (None = now). Returns a CUDA uint8 tensor of
+    exactly the archive's length. Raises on any error, as check() does."""
+    import time
+    import torch
+    lib = load()
+    check(lib.mz_cuda_init(), "mz_cuda_init")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    flags = (MZ_ZIP_CUDA_HASH_SHA256 if sha256 else 0) | (MZ_ZIP_CUDA_AES if password is not None else 0)
+    date = dos_date(int(time.time() if mtime is None else mtime))
+    tensors = []
+    for name, t in files:
+        assert t.is_cuda and t.dtype == torch.uint8 and t.device == dev, "%s: a CUDA uint8 tensor on the current device" % name
+        tensors.append(t.contiguous())
+    ptrs = [t.data_ptr() for t in tensors if t.numel()]
+    base = min(ptrs) if ptrs else 0
+    names = [n.encode() for n, _ in files]
+    blob = b"".join(names)
+    d_names = torch.frombuffer(bytearray(blob or b"\0"), dtype=torch.uint8).to(dev)
+    items = (ZipDevItem * max(1, len(files)))()
+    pos = 0
+    for i, (nm, t) in enumerate(zip(names, tensors)):
+        items[i] = ZipDevItem(t.data_ptr() - base if t.numel() else 0, t.numel(), pos, len(nm), date, 0, 0)
+        pos += len(nm)
+    d_items = torch.frombuffer(bytearray(bytes(items)), dtype=torch.uint8).to(dev)
+    pw = password.encode() if password is not None else None
+    s = _stream_ptr()
+    n = C.c_uint64(0)
+    args = (base or None, d_names.data_ptr(), d_items.data_ptr(), len(files), level, flags, pw, aes_strength)
+    check(lib.mz_zip_cuda_write_device(*args, None, 0, C.byref(n), None, None, s), "write_device")  # sizing: an upper bound
+    out = torch.empty(max(1, n.value), dtype=torch.uint8, device=dev)
+    check(lib.mz_zip_cuda_write_device(*args, out.data_ptr(), n.value, C.byref(n), None, None, s), "write_device")
+    return out[:n.value].clone()  # the bound-sized buffer is released: the archive's own storage is exactly its length
 
 
 def inflate_device(comp, out_cap):

@@ -20,6 +20,7 @@
 #include "wzaes_kernel.cuh"
 #include "zipdir_kernel.cuh"
 #include "zipcd_kernel.cuh"
+#include "zipwr_kernel.cuh"
 #include "../../include/mz_zip_cuda.h"
 
 #define MZ_OK 0
@@ -39,6 +40,10 @@ static_assert(sizeof(mz_cuda_zip_round) == sizeof(ZipRound), "zip round layout")
 static_assert(sizeof(mz_cuda_zip_dev_entry) == sizeof(ZipDevEnt) && sizeof(mz_cuda_zip_dev_entry) == 72 &&
                   offsetof(mz_cuda_zip_dev_entry, status) == offsetof(ZipDevEnt, status) && offsetof(ZipDevEnt, status) == 68,
               "device zip entry layout");
+static_assert(sizeof(mz_cuda_zip_dev_item) == sizeof(ZwItem) && sizeof(ZwItem) == 40 && sizeof(mz_cuda_zip_wr_count) == sizeof(ZwCount) &&
+                  sizeof(mz_cuda_zip_wr) == sizeof(ZwCall) && offsetof(mz_cuda_zip_wr, entries) == offsetof(ZwCall, entries) &&
+                  MZ_CUDA_ZIP_WR_TILE == ZC_TILE,
+              "device zip writer layout");
 
 namespace {
 
@@ -708,6 +713,95 @@ int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entri
     if (n == 0) return MZ_OK;
     if (!d_status || !d_entries || !d_first) return MZ_PARAM_ERROR;
     MZ_LAUNCH(zc_status_kernel, dim3(zc_grid(n)), dim3(ZC_THREADS), 0, (cudaStream_t)stream, d_status, n, (ZipDevEnt *)d_entries, d_first);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+/* ---- K11: a zip archive written into device memory -------------------------------------------------------------- */
+extern "C++" {
+namespace {
+ZwCall zw_call(const mz_cuda_zip_wr *w) {
+    ZwCall W;
+    memcpy(&W, w, sizeof(W));
+    return W;
+}
+/* out[i] = in[0] + ... + in[i-1] for i = 0..n, with the tiles' sums in part (n / ZC_TILE + 1 of them) */
+template <typename T> int32_t zw_scan(const T *in, uint64_t n, T *out, T *part, cudaStream_t s) {
+    const uint64_t nb = n / ZC_TILE + 1;
+    MZ_LAUNCH(zc_scan_reduce_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, s, in, n, part);
+    MZ_LAUNCH(zc_scan_parts_kernel<T>, dim3(1), dim3(ZC_THREADS), 0, s, part, (uint32_t)nb);
+    MZ_LAUNCH(zc_scan_apply_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, s, in, n, (const T *)part, out);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+} // namespace
+} // extern "C++"
+
+int32_t mz_cuda_zip_wr_items(const mz_cuda_zip_wr *w, uint32_t data_null, uint32_t names_null, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!w || !w->cnt || !w->pre || !w->part || !w->bad || (w->n && !w->items)) return MZ_PARAM_ERROR;
+    const ZwCall W = zw_call(w);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (W.n) MZ_LAUNCH(zw_items_kernel, dim3((W.n + ZW_THREADS - 1) / ZW_THREADS), dim3(ZW_THREADS), 0, s, W, data_null, names_null);
+    CK(cudaGetLastError());
+    return zw_scan<ZwCount>(W.cnt, W.n, W.pre, (ZwCount *)W.part, s);
+}
+
+int32_t mz_cuda_zip_wr_chunks(const mz_cuda_zip_wr *w, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!w || !w->c_off || !w->c_len || !w->c_flags || !w->c_item || (w->sha && (!w->e_off || !w->e_len))) return MZ_PARAM_ERROR;
+    if (w->nch == 0) return MZ_OK;
+    const uint64_t g = (w->nch + ZW_THREADS - 1) / ZW_THREADS;
+    if (g > 0x7fffffffull) return MZ_SUPPORT_ERROR;
+    MZ_LAUNCH(zw_chunks_kernel, dim3((uint32_t)g), dim3(ZW_THREADS), 0, (cudaStream_t)stream, zw_call(w));
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_wr_place(const mz_cuda_zip_wr *w, uint64_t c0, uint32_t m, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!w || !w->out_len || !w->S || !w->dst || !w->glen || !w->part || m > 32768u || c0 + m > w->nch) return MZ_PARAM_ERROR;
+    if (m == 0) return MZ_OK;
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t nb = m / ZC_TILE + 1;
+    uint32_t *part = (uint32_t *)w->part;
+    /* the round's stream bytes fit 32 bits: at most 32768 chunks of mz_cuda_deflate_slot_bound(65536) each */
+    MZ_LAUNCH(zc_scan_reduce_kernel<uint32_t>, dim3(nb), dim3(ZC_THREADS), 0, s, (const uint32_t *)w->out_len + c0, (uint64_t)m, part);
+    MZ_LAUNCH(zc_scan_parts_kernel<uint32_t>, dim3(1), dim3(ZC_THREADS), 0, s, part, nb);
+    MZ_LAUNCH(zw_place_kernel, dim3(nb), dim3(ZC_THREADS), 0, s, zw_call(w), c0, m, (const uint32_t *)part);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_wr_entries(const mz_cuda_zip_wr *w, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!w || !w->e_lh || !w->e_csize || !w->e_cd || !w->e_cdpre || !w->e_coff || !w->e_crc || !w->max_csize || !w->residue || !w->S) return MZ_PARAM_ERROR;
+    const ZwCall W = zw_call(w);
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t per = ZW_THREADS / 32;
+    if (W.n) MZ_LAUNCH(zw_entries_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, (const CrcConsts *)c->d_consts);
+    CK(cudaGetLastError());
+    return zw_scan<uint64_t>(W.e_cd, W.n, W.e_cdpre, (uint64_t *)W.part, s);
+}
+
+int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t cd_size, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!w || !w->archive || (w->sha && !w->digest) || (w->aes && (!w->salt || !w->keys || !w->mac))) return MZ_PARAM_ERROR;
+    const ZwCall W = zw_call(w);
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t per = ZW_THREADS / 32;
+    if (W.n) MZ_LAUNCH(zw_emit_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, cd_off);
+    MZ_LAUNCH(zw_end_kernel, dim3(1), dim3(1), 0, s, W, cd_off, cd_size);
     CK(cudaGetLastError());
     return MZ_OK;
 }

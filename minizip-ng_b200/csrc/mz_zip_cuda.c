@@ -2095,3 +2095,194 @@ int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const ch
         *stats = st;
     return err;
 }
+
+/* ---- an archive written into device memory (mz_zip_cuda_write_device) ---------------------------------------------------- */
+/* carve sizes[k] bytes per piece from one device allocation (256-byte aligned pieces); NULL when it fails */
+static uint8_t *zw_carve(const size_t *sz, void **out[], int k) {
+    size_t off[32], total = 0;
+    for (int i = 0; i < k; i++) {
+        off[i] = total;
+        total += (sz[i] + 255) & ~(size_t)255;
+    }
+    uint8_t *w = (uint8_t *)mz_cuda_malloc(total);
+    if (!w)
+        return NULL;
+    for (int i = 0; i < k; i++)
+        *out[i] = w + off[i];
+    return w;
+}
+
+int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags,
+                                 const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
+                                 mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    /* the host writer's order: options, pointers, level, password and strength, the GPU */
+    if (flags & ~(MZ_ZIP_CUDA_HASH_SHA256 | MZ_ZIP_CUDA_AES))
+        return MZ_PARAM_ERROR; /* MZ_ZIP_CUDA_ALL_DEVICES among them: the entries live on one device */
+    if (!archive_len || (!d_items && count))
+        return MZ_PARAM_ERROR;
+    *archive_len = 0;
+    if (level == MZ_COMPRESS_LEVEL_DEFAULT)
+        level = 6;
+    if (level < 0 || level > 9)
+        return MZ_PARAM_ERROR;
+    const int aes = (flags & MZ_ZIP_CUDA_AES) != 0;
+    if (aes_strength == 0)
+        aes_strength = 3;
+    if (aes && (!password || strlen(password) > 128 || aes_strength > 3))
+        return MZ_PARAM_ERROR;
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    const double t0 = now_ms();
+    mz_cuda_zip_wr w;
+    memset(&w, 0, sizeof(w));
+    w.data = d_data;
+    w.names = d_names;
+    w.items = d_items;
+    w.n = count;
+    w.aes = aes ? aes_strength : 0;
+    w.sha = (flags & MZ_ZIP_CUDA_HASH_SHA256) != 0;
+    w.dos_now = za_dos_date(0);
+    w.archive = d_archive;
+    w.cap = d_archive ? cap : 0;
+    w.entries = d_entries;
+    const size_t m = (size_t)count + 1, tiles = (size_t)count / MZ_CUDA_ZIP_WR_TILE + 1;
+    /* 1. validation and per-item counts: the first invalid item and the totals come back */
+    const size_t sz1[4] = {16, m * sizeof(mz_cuda_zip_wr_count), m * sizeof(mz_cuda_zip_wr_count), tiles * sizeof(mz_cuda_zip_wr_count)};
+    void **p1[4] = {(void **)&w.bad, (void **)&w.cnt, (void **)&w.pre, &w.part};
+    double ts = now_ms();
+    uint8_t *work1 = zw_carve(sz1, p1, 4), *work2 = NULL;
+    st.setup_ms += now_ms() - ts;
+    if (!work1)
+        return MZ_MEM_ERROR;
+    int32_t err = mz_cuda_memset(w.bad, 0xff, 8, stream);
+    if (!err) err = mz_cuda_zip_wr_items(&w, d_data == NULL, d_names == NULL, stream);
+    uint64_t bad = ~0ull;
+    mz_cuda_zip_wr_count tot;
+    memset(&tot, 0, sizeof(tot));
+    if (!err) err = mz_cuda_memcpy_d2h(&bad, w.bad, 8, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&tot, w.pre + count, sizeof(tot), stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    if (!err && bad != ~0ull)
+        err = (bad & 1) ? MZ_SUPPORT_ERROR : MZ_PARAM_ERROR;
+    if (!err && !d_archive) { /* sizing: the slot bound of every chunk, exact headers; the zip64 fields only when an offset can need them */
+        const int big = tot.overhead + tot.bound >= 0xffffffffull;
+        *archive_len = tot.overhead + tot.bound + tot.cd + (big ? 28ull * count : 0) + 22 + (big || count >= 0xffffu ? 76 : 0);
+    }
+    st.pack_ms = now_ms() - t0 - st.setup_ms; /* the scratch allocation is setup_ms */
+    if (err || !d_archive) {
+        mz_cuda_stream_sync(stream);
+        mz_cuda_free(work1);
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    /* 2. scratch: the chunk table, a round of slots, per-entry arrays */
+    size_t round_bytes = (size_t)1024 << 20;
+    {
+        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
+        if (v && atoll(v) > 0)
+            round_bytes = (size_t)atoll(v) << 20;
+    }
+    uint64_t R = round_bytes / ZC_CHUNK; /* chunks per round: every chunk holds at most 64 KiB */
+    if (R < 1) R = 1;
+    if (R > 32768) R = 32768;
+    w.nch = tot.chunks;
+    if (R > w.nch) R = w.nch ? w.nch : 1;
+    const uint64_t stride = mz_cuda_deflate_slot_bound(ZC_CHUNK);
+    const size_t nch = (size_t)w.nch, n = count ? count : 1;
+    const size_t ptiles = ((size_t)R > n ? (size_t)R : n) / MZ_CUDA_ZIP_WR_TILE + 1;
+    uint8_t *slots = NULL, *pw = NULL;
+    void *digest = NULL, *salt = NULL, *keys = NULL, *mac = NULL;
+    const size_t sz2[26] = {nch * 8, nch * 4, nch, nch * 4, nch * 4, nch * 4, nch * 4, (nch + 1) * 8, nch * 8,
+                            n * 8, n * 8, n * 8, (n + 1) * 8, n * 8, n * 8, n * 8, n * 4, 8, ptiles * sizeof(mz_cuda_zip_wr_count),
+                            (size_t)R * stride, w.sha ? n * 32 : 32, aes ? n * 16 : 16, aes ? n * MZ_CUDA_WZAES_KEYREC : 16, aes ? n * 20 : 16, 256,
+                            16};
+    void *part2 = NULL, *spare = NULL;
+    void **p2[26] = {(void **)&w.c_off, (void **)&w.c_len, (void **)&w.c_flags, (void **)&w.c_item, (void **)&w.out_len, (void **)&w.residue, (void **)&w.glen,
+                     (void **)&w.S, (void **)&w.dst, (void **)&w.e_lh, (void **)&w.e_csize, (void **)&w.e_cd, (void **)&w.e_cdpre, (void **)&w.e_coff,
+                     (void **)&w.e_off, (void **)&w.e_len, (void **)&w.e_crc, (void **)&w.max_csize, &part2, (void **)&slots, &digest, &salt, &keys, &mac,
+                     (void **)&pw, &spare};
+    ts = now_ms();
+    work2 = zw_carve(sz2, p2, 26);
+    st.setup_ms += now_ms() - ts;
+    if (!work2)
+        err = MZ_MEM_ERROR;
+    w.part = part2;
+    w.digest = digest;
+    w.salt = salt;
+    w.keys = keys;
+    w.mac = mac;
+    /* 3. the chunk table; SHA-256 of every entry (K7) */
+    const double t1 = now_ms();
+    if (!err) err = mz_cuda_memset(w.S, 0, 8, stream);
+    if (!err) err = mz_cuda_memset(w.max_csize, 0, 8, stream);
+    if (!err) err = mz_cuda_zip_wr_chunks(&w, stream);
+    if (!err && w.sha) err = mz_cuda_sha256_batch(d_data ? d_data : digest, w.e_off, w.e_len, count, digest, stream);
+    /* 4. rounds over the global chunk list: compress, checksum, place, gather into the archive; no host synchronisation between */
+    for (uint64_t c0 = 0; !err && c0 < w.nch; c0 += R) {
+        const uint32_t mr = (uint32_t)(w.nch - c0 < R ? w.nch - c0 : R);
+        err = mz_cuda_deflate_chunks(d_data, 0, 0, w.c_off + c0, w.c_len + c0, w.c_flags + c0, mr, 0, level, slots, stride, w.out_len + c0, stream);
+        if (!err) err = mz_cuda_crc32_segments(d_data, 0, 0, w.c_off + c0, w.c_len + c0, mr, w.residue + c0, NULL, stream);
+        if (!err) err = mz_cuda_zip_wr_place(&w, c0, mr, stream);
+        if (!err) err = mz_cuda_gather(slots, stride, w.glen + c0, mr, w.dst + c0, d_archive, stream);
+        st.rounds++;
+    }
+    /* 5. per entry: CRC, sizes, offsets, directory layout; the exact length comes back */
+    if (!err) err = mz_cuda_zip_wr_entries(&w, stream);
+    uint64_t streams = 0, cd_size = 0, max_csize = 0;
+    if (!err) err = mz_cuda_memcpy_d2h(&streams, w.S + w.nch, 8, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&cd_size, w.e_cdpre + count, 8, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&max_csize, w.max_csize, 8, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&bad, w.bad, 8, stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    const uint64_t cd_off = tot.overhead + streams;
+    const uint64_t len = cd_off + cd_size + 22 + (cd_off >= 0xffffffffull || count >= 0xffffu ? 76 : 0);
+    if (!err && bad != ~0ull)
+        err = MZ_INTERNAL_ERROR; /* an entry's stored size does not fit its local header: what za_prepare returns for it */
+    if (!err) {
+        *archive_len = len;
+        if (len > cap)
+            err = MZ_BUF_ERROR;
+    }
+    /* 6. WinZip AES: fresh salts from the host, keys by K8, the streams encrypted in place, their HMACs; then headers, directory,
+     * end records and the table */
+    if (!err && aes && count) {
+        uint8_t *h_salt = (uint8_t *)malloc((size_t)count * 16);
+        size_t got = 0;
+        if (!h_salt)
+            err = MZ_MEM_ERROR;
+        while (!err && got < (size_t)count * 16) {
+            ssize_t k = getrandom(h_salt + got, (size_t)count * 16 - got, 0);
+            if (k <= 0) { err = MZ_INTERNAL_ERROR; break; }
+            got += (size_t)k;
+        }
+        const uint32_t pwl = (uint32_t)strlen(password);
+        if (!err) err = mz_cuda_memcpy_h2d(salt, h_salt, (size_t)count * 16, stream);
+        if (!err) err = mz_cuda_memcpy_h2d(pw, password, pwl ? pwl : 1, stream);
+        if (!err) err = mz_cuda_stream_sync(stream); /* the pageable sources are freed below */
+        free(h_salt);
+        if (!err) err = mz_cuda_wzaes_derive(pw, pwl, salt, count, aes_strength, keys, stream);
+        if (!err) err = mz_cuda_wzaes_ctr(d_archive, w.e_coff, w.e_csize, count, max_csize, keys, aes_strength, stream);
+        if (!err) err = mz_cuda_wzaes_hmac(d_archive, w.e_coff, w.e_csize, count, keys, aes_strength, mac, stream);
+    }
+    if (!err) err = mz_cuda_zip_wr_emit(&w, cd_off, cd_size, stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    st.gpu_ms = now_ms() - t1;
+    if (!err || err == MZ_BUF_ERROR) {
+        st.entries = count;
+        st.bytes_in = tot.bytes;
+        st.bytes_out = streams + (aes ? (uint64_t)count * (4u * aes_strength + 4u + 2u + 10u) : 0);
+    }
+    mz_cuda_stream_sync(stream);
+    mz_cuda_free(work2);
+    mz_cuda_free(work1);
+    if (stats)
+        *stats = st;
+    return err;
+}
