@@ -235,11 +235,56 @@ typedef struct mz_cuda_zip_dir {
     uint64_t cd_off, out_bytes, bytes_in, bytes_out, max_clen[4];
     mz_cuda_zip_ent *ent;
     void *sha_expect;
+    /* in: with entries == NULL, allocate the public table (count rows) when it fits and set entries to it; the caller frees it
+     * with mz_cuda_free (the reader of mz_zip_cuda_reader_open keeps it) */
+    uint32_t alloc_entries, pad2;
 } mz_cuda_zip_dir;
 int32_t mz_cuda_zip_parse_directory(const void *d_archive, uint64_t len, mz_cuda_zip_dir *dir, void *stream);
 /* after mz_cuda_zip_verify: each entry's status (0 or -MZ code) into the mz_cuda_zip_dev_entry table, and *d_first lowered to the
  * index of the first failing entry (the caller sets it to 0xffffffff first) */
 int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entries, uint32_t *d_first, void *stream);
+
+/* ---- K12: random access to an archive in device memory (csrc/zipsel_kernel.cuh) ---------------------------------------
+ * The device half of the reader (mz_zip_cuda_reader_*, include/mz_zip_cuda.h). Name index: d_table holds P slots (a power of
+ * two >= 2 x n, every slot ~0 before the build) of hash tag << 32 | entry index; the build inserts every one of the n entries of
+ * the public table (names read from d_archive). Lookup: one thread per query (d_names + d_name_off[q], d_name_len[q] bytes);
+ * d_index[q] = the smallest entry index whose name equals the query under mz_zip_path_compare(name, query, ignore_case), or
+ * 0xffffffff. A lookup costs its probe length plus one compare per entry whose folded name hashes the same. P = 0: every query
+ * misses. */
+int32_t mz_cuda_zip_name_index(const void *d_archive, const void *d_entries, uint32_t n, uint64_t *d_table, uint32_t P, void *stream);
+int32_t mz_cuda_zip_name_lookup(const void *d_archive, const void *d_entries, const uint64_t *d_table, uint32_t P, const void *d_names,
+                                const uint64_t *d_name_off, const uint32_t *d_name_len, uint32_t nq, uint8_t ignore_case, uint32_t *d_index,
+                                void *stream);
+/* A selection of n slots, slot i = entry select[i] of the archive-wide K9 table ent (count rows, src_off / src_len = local header
+ * and extent in the archive). count: per-slot counts and their exclusive scan pre[0..n] (part: scan scratch of n /
+ * MZ_CUDA_ZIP_WR_TILE + 1 rows). fill: out_off[0..n] (if not NULL) and, with sel, the selection's K9 records (src_off in scratch
+ * at pre.gather when gather is set, otherwise in the archive); an index >= count gets an inert record. gather: every valid
+ * slot's extent to scratch + pre.gather. status: after mz_cuda_zip_verify, out[i] (if not NULL) = slot i's MZ code
+ * (MZ_END_OF_LIST for an index >= count), *d_first (~0 before) lowered to slot << 32 | -code of the first failing slot. */
+typedef struct mz_cuda_zip_sel_count { /* per slot; pre[i] = the sum over the slots in front of i */
+    uint64_t out;       /* plain bytes rounded up to 16 */
+    uint64_t cin, cout; /* stored and plain bytes */
+    uint64_t gather;    /* extent rounded up to 16 */
+    uint32_t job, sha;  /* DEFLATE (K5 job), an expected SHA-256 */
+    uint32_t a[4];      /* a[s]: WinZip AES strength s */
+} mz_cuda_zip_sel_count;
+typedef struct mz_cuda_zip_sel {
+    const void *archive;
+    const mz_cuda_zip_ent *ent;
+    uint32_t count, n;
+    const uint32_t *select;
+    mz_cuda_zip_sel_count *cnt, *pre;
+    void *part;
+    uint32_t gather, pad;
+    mz_cuda_zip_ent *sel;
+    uint64_t *out_off;
+    void *scratch;
+} mz_cuda_zip_sel;
+int32_t mz_cuda_zip_sel_counts(const mz_cuda_zip_sel *c, void *stream);
+int32_t mz_cuda_zip_sel_fill(const mz_cuda_zip_sel *c, void *stream);
+int32_t mz_cuda_zip_sel_gather(const mz_cuda_zip_sel *c, void *stream);
+int32_t mz_cuda_zip_sel_status(const uint32_t *d_status, const uint32_t *d_select, uint32_t n, uint32_t count, int32_t *d_out, uint64_t *d_first,
+                               void *stream);
 
 /* ---- K11: a zip archive written into device memory (csrc/zipwr_kernel.cuh) --------------------------------------------
  * The device half of mz_zip_cuda_write_device (include/mz_zip_cuda.h). One call state, device pointers unless noted; the host

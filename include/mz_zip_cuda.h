@@ -167,6 +167,55 @@ typedef struct mz_cuda_zip_dev_entry {
 int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
                                    uint32_t *count, void *d_out, uint64_t out_cap, uint64_t *out_bytes, mz_cuda_zip_stats *stats, void *stream);
 
+/* ---- random access to an archive in device memory ----------------------------------------------------------------------
+ * A reader parses the directory of an archive in device memory once and then looks entries up by name and decodes any chosen
+ * subset of them, many times: what mz_zip_locate_entry (mz_zip.c:2414) and mz_zip_entry_read_* do entry by entry in the
+ * reference, for batches of entries on the device (K10 at open, K12 for the name index and the selections, K9 / K8 / K5 / K1 / K7
+ * for the decode, csrc/zipsel_kernel.cuh).
+ *
+ * open: parses the directory (K10, once) and builds the name index. An error of the archive as a whole is returned exactly as
+ *   mz_zip_cuda_extract_device returns it, and no reader is created. Otherwise MZ_OK with *count = the records accepted and
+ *   *refuse = the error that ended the list or MZ_OK (what extract_device returns after listing). The password (may be NULL) is
+ *   copied. The archive must stay allocated and unchanged while the reader is open; the reader never writes it. A reader belongs
+ *   to the device current at open and serves one call at a time; readers are independent of each other. stats (may be NULL):
+ *   entries / bytes_in / bytes_out of the accepted entries, pack_ms = the directory parse, gpu_ms = the index build, setup_ms =
+ *   the index allocation.
+ * entries: the device table of the *count accepted records, row for row what extract_device lists (out_off included, status 0).
+ * locate: enqueued on `stream`, no host synchronisation (its output can feed decode directly). Query q is the d_name_len[q] bytes
+ *   at d_names + d_name_off[q], all in device memory. d_index[q] = the first accepted entry in directory order whose name compares
+ *   equal to the query under mz_zip_path_compare(name, query, ignore_case) (mz_zip.c:2754): both taken as C strings (the bytes
+ *   before the first NUL), '\\' equal to '/', with ignore_case only A-Z folded (tolower in the C locale; bytes >= 0x80 compare
+ *   exactly). No match, or an empty query: 0xffffffff. Unlike the reference, whose walk continues past the records this library
+ *   refuses, a name behind the record that ended the list is not found. Cost: a hash-table probe per query plus one compare per
+ *   entry whose folded name hashes the same (all duplicates of a name).
+ * decode: synchronous on `stream`. Slot i decodes entry d_select[i]; any selection is valid (repeats, any order, nsel = 0). The
+ *   plain bytes are packed in selection order, each at a 16-byte aligned offset; d_out_off (optional, nsel + 1 values) receives
+ *   the offsets and the total, *out_bytes the total.
+ *   - MZ_PARAM_ERROR first: a NULL reader or out_bytes, d_select NULL with nsel > 0, d_out not 16-byte aligned;
+ *   - d_out == NULL: sizing call: *out_bytes and d_out_off are set, nothing is decoded;
+ *   - out_cap < *out_bytes: MZ_BUF_ERROR with *out_bytes set; nothing is written to d_out, d_out_off or d_status;
+ *   - otherwise every slot is decoded and verified exactly as extract_device does it (local header, AES verifier and HMAC, DEFLATE
+ *     end state and sizes, CRC-32, SHA-256): its bytes and status equal those extract_device gives that entry. An index >= count
+ *     gets MZ_END_OF_LIST (what mz_zip_locate_entry returns for a missing name, so a miss from locate passes straight through)
+ *     and no bytes. d_status (optional, nsel values) receives every slot's status; the return value is the status of the first
+ *     failing slot in selection order, or MZ_OK.
+ *   WinZip AES entries are decrypted in place by K8, so a selection that holds any is first gathered (every slot's extent) into
+ *   scratch the reader owns; the same entry selected twice is decrypted once per slot. The reader keeps its scratch between calls
+ *   and grows it only when a selection needs more. Host synchronisation: one readback of the selection's totals before the decode
+ *   launches and one of the first failing slot after it. stats (may be NULL): entries / bytes_in / bytes_out of the valid slots,
+ *   pack_ms = to the first readback, gpu_ms = decode and verify, setup_ms = scratch allocation (0 when the scratch fitted).
+ * close: frees everything the reader allocated (NULL is a no-op).
+ * Entries above 1 GiB are refused at open as extract_device refuses them. */
+typedef struct mz_zip_cuda_dev_reader mz_zip_cuda_dev_reader;
+int32_t mz_zip_cuda_reader_open(const void *d_archive, uint64_t len, const char *password, mz_zip_cuda_dev_reader **reader, uint32_t *count,
+                                int32_t *refuse, mz_cuda_zip_stats *stats, void *stream);
+const mz_cuda_zip_dev_entry *mz_zip_cuda_reader_entries(const mz_zip_cuda_dev_reader *reader);
+int32_t mz_zip_cuda_reader_locate(mz_zip_cuda_dev_reader *reader, const void *d_names, const uint64_t *d_name_off, const uint32_t *d_name_len,
+                                  uint32_t n, uint8_t ignore_case, uint32_t *d_index, void *stream);
+int32_t mz_zip_cuda_reader_decode(mz_zip_cuda_dev_reader *reader, const uint32_t *d_select, uint32_t nsel, void *d_out, uint64_t out_cap,
+                                  uint64_t *out_bytes, uint64_t *d_out_off, int32_t *d_status, mz_cuda_zip_stats *stats, void *stream);
+void mz_zip_cuda_reader_close(mz_zip_cuda_dev_reader *reader);
+
 /* ---- an archive written into device memory from entries in device memory ---------------------------------------------
  * The archive mz_zip_cuda_write_archive (flags with MZ_ZIP_CUDA_AES: mz_zip_cuda_write_archive_aes) writes for the same entries,
  * level, flags and dates, byte for byte (with AES only the random salts and what follows from them differ), built in device memory

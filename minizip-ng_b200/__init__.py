@@ -59,10 +59,14 @@ EXPORTS = [
     # include/mz_zip_cuda.h
     "mz_zip_cuda_add_buffers", "mz_zip_cuda_add_buffers_ex", "mz_zip_cuda_write_archive", "mz_zip_cuda_trim", "mz_zip_cuda_write_archive_aes", "mz_zip_cuda_extract_all",
     "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_extract_device", "mz_zip_cuda_write_device", "mz_zip_cuda_abi_file_info_size",
+    "mz_zip_cuda_reader_open", "mz_zip_cuda_reader_entries", "mz_zip_cuda_reader_locate", "mz_zip_cuda_reader_decode", "mz_zip_cuda_reader_close",
     # include/mz_cuda_batch.h, K9 and K10
     "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify", "mz_cuda_zip_parse_directory", "mz_cuda_zip_statuses",
     # include/mz_cuda_batch.h, K11
     "mz_cuda_zip_wr_items", "mz_cuda_zip_wr_chunks", "mz_cuda_zip_wr_place", "mz_cuda_zip_wr_entries", "mz_cuda_zip_wr_emit",
+    # include/mz_cuda_batch.h, K12
+    "mz_cuda_zip_name_index", "mz_cuda_zip_name_lookup", "mz_cuda_zip_sel_counts", "mz_cuda_zip_sel_fill", "mz_cuda_zip_sel_gather",
+    "mz_cuda_zip_sel_status",
 ]
 
 # mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
@@ -193,6 +197,17 @@ def configure(L):
     sig("mz_zip_cuda_write_device", i32, [vp, vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp, u64, C.POINTER(u64), vp, vp, vp])
     sig("mz_cuda_zip_parse_directory", i32, [vp, u64, vp, vp])
     sig("mz_cuda_zip_statuses", i32, [vp, u32, vp, vp, vp])
+    sig("mz_zip_cuda_reader_open", i32, [vp, u64, C.c_char_p, C.POINTER(vp), C.POINTER(u32), C.POINTER(i32), vp, vp])
+    sig("mz_zip_cuda_reader_entries", vp, [vp])
+    sig("mz_zip_cuda_reader_locate", i32, [vp, vp, vp, vp, u32, C.c_uint8, vp, vp])
+    sig("mz_zip_cuda_reader_decode", i32, [vp, vp, u32, vp, u64, C.POINTER(u64), vp, vp, vp, vp])
+    sig("mz_zip_cuda_reader_close", None, [vp])
+    sig("mz_cuda_zip_name_index", i32, [vp, vp, u32, vp, u32, vp])
+    sig("mz_cuda_zip_name_lookup", i32, [vp, vp, vp, u32, vp, vp, vp, u32, C.c_uint8, vp, vp])
+    sig("mz_cuda_zip_sel_counts", i32, [vp, vp])
+    sig("mz_cuda_zip_sel_fill", i32, [vp, vp])
+    sig("mz_cuda_zip_sel_gather", i32, [vp, vp])
+    sig("mz_cuda_zip_sel_status", i32, [vp, vp, u32, u32, vp, vp, vp])
     return L
 
 
@@ -302,6 +317,98 @@ def extract_device(archive, password=None):
         names = archive[lo:max(r.name_off + r.name_len for r in rows)].cpu().numpy().tobytes()
         entries = [(names[r.name_off - lo:r.name_off - lo + r.name_len].decode("utf-8", "replace"), r.out_off, r.usize, r.crc) for r in rows]
     return entries, out[:nbytes.value]
+
+
+class ZipDeviceReader:
+    """Random access to a zip archive held in a CUDA uint8 tensor (mz_zip_cuda_reader_*): the directory is parsed once on the device,
+    entries are looked up by name and any subset of them decoded on the device, as often as needed. The tensor must stay unchanged
+    while the reader is open; the reader never writes it.
+
+    .entries: [(name, size, crc)] of the accepted entries in directory order (read once at open); .refuse: the error that ended the
+    list, or MZ_OK. .locate(names, ignore_case=False): a CUDA int64 tensor of entry indices, -1 for a miss. .read(indices): decodes
+    the entries (a CUDA or CPU integer tensor, or a list; repeats and any order allowed) and returns (offsets, out) as CUDA tensors:
+    entry k of the selection is out[offsets[k]:offsets[k] + size]. Errors raise, as extract_device's do. .close() or `with`."""
+
+    def __init__(self, archive, password=None):
+        import torch
+        self.lib = load()
+        check(self.lib.mz_cuda_init(), "mz_cuda_init")
+        assert archive.is_cuda and archive.dtype == torch.uint8, "archive: a CUDA uint8 tensor"
+        self.archive = archive.contiguous()  # kept: the reader reads it until close
+        self.device = self.archive.device
+        self._r = C.c_void_p()
+        n = self.archive.numel()
+        count, refuse = C.c_uint32(0), C.c_int32(0)
+        with torch.cuda.device(self.device):
+            check(self.lib.mz_zip_cuda_reader_open(self.archive.data_ptr() if n else None, n, password.encode() if password is not None else None,
+                                                   C.byref(self._r), C.byref(count), C.byref(refuse), None, _stream_ptr()), "reader_open")
+        self.count, self.refuse = count.value, refuse.value
+        self._rows = []
+        self.entries = []
+        if self.count:
+            table = torch.empty(self.count * C.sizeof(ZipDevEntry), dtype=torch.uint8, device=self.device)
+            check(self.lib.mz_cuda_memcpy_d2d(table.data_ptr(), self.lib.mz_zip_cuda_reader_entries(self._r), table.numel(), _stream_ptr()), "entries")
+            self._rows = (ZipDevEntry * self.count).from_buffer_copy(table.cpu().numpy().tobytes())
+            lo = min(r.name_off for r in self._rows)
+            names = self.archive[lo:max(r.name_off + r.name_len for r in self._rows)].cpu().numpy().tobytes()
+            self.entries = [(names[r.name_off - lo:r.name_off - lo + r.name_len].decode("utf-8", "replace"), r.usize, r.crc) for r in self._rows]
+
+    def _live(self):
+        if not self._r:
+            raise RuntimeError("ZipDeviceReader is closed")
+
+    def locate(self, names, ignore_case=False):
+        import torch
+        self._live()
+        raw = [n.encode() if isinstance(n, str) else bytes(n) for n in names]
+        out = torch.empty(max(1, len(raw)), dtype=torch.int32, device=self.device)
+        if raw:
+            blob = b"".join(raw) or b"\0"
+            offs, pos = [], 0
+            for r in raw:
+                offs.append(pos)
+                pos += len(r)
+            d_names = torch.frombuffer(bytearray(blob), dtype=torch.uint8).to(self.device)
+            d_off = torch.tensor(offs, dtype=torch.int64, device=self.device)
+            d_len = torch.tensor([len(r) for r in raw], dtype=torch.int32, device=self.device)
+            with torch.cuda.device(self.device):
+                check(self.lib.mz_zip_cuda_reader_locate(self._r, d_names.data_ptr(), d_off.data_ptr(), d_len.data_ptr(), len(raw), 1 if ignore_case else 0,
+                                                         out.data_ptr(), _stream_ptr()), "reader_locate")
+        return out[:len(raw)].to(torch.int64)  # a miss, 0xffffffff, reads as -1
+
+    def read(self, indices):
+        import torch
+        self._live()
+        sel = torch.as_tensor(indices, dtype=torch.int64).to(self.device).reshape(-1)
+        # an index outside the entries (a miss from locate included) becomes 0xffffffff: the decode reports MZ_END_OF_LIST for it
+        d_sel = torch.where((sel < 0) | (sel >= self.count), torch.full_like(sel, -1), sel).to(torch.int32)
+        n = d_sel.numel()
+        offs = torch.empty(n + 1, dtype=torch.int64, device=self.device)
+        size = C.c_uint64(0)
+        s = _stream_ptr()
+        with torch.cuda.device(self.device):
+            check(self.lib.mz_zip_cuda_reader_decode(self._r, d_sel.data_ptr() if n else None, n, None, 0, C.byref(size), None, None, None, s), "reader_decode")
+            out = torch.empty(max(16, size.value), dtype=torch.uint8, device=self.device)
+            check(self.lib.mz_zip_cuda_reader_decode(self._r, d_sel.data_ptr() if n else None, n, out.data_ptr(), size.value, C.byref(size),
+                                                     offs.data_ptr(), None, None, s), "reader_decode")
+        return offs, out[:size.value]
+
+    def close(self):
+        if self._r:
+            self.lib.mz_zip_cuda_reader_close(self._r)
+            self._r = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001 -- interpreter shutdown
+            pass
 
 
 def write_device(files, level=6, sha256=False, password=None, aes_strength=3, mtime=None):

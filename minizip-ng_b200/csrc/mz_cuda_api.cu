@@ -21,6 +21,7 @@
 #include "zipdir_kernel.cuh"
 #include "zipcd_kernel.cuh"
 #include "zipwr_kernel.cuh"
+#include "zipsel_kernel.cuh"
 #include "../../include/mz_zip_cuda.h"
 
 #define MZ_OK 0
@@ -44,6 +45,9 @@ static_assert(sizeof(mz_cuda_zip_dev_item) == sizeof(ZwItem) && sizeof(ZwItem) =
                   sizeof(mz_cuda_zip_wr) == sizeof(ZwCall) && offsetof(mz_cuda_zip_wr, entries) == offsetof(ZwCall, entries) &&
                   MZ_CUDA_ZIP_WR_TILE == ZC_TILE,
               "device zip writer layout");
+static_assert(sizeof(mz_cuda_zip_sel_count) == sizeof(ZsCount) && sizeof(ZsCount) == 56 && sizeof(mz_cuda_zip_sel) == sizeof(ZsCall) &&
+                  offsetof(mz_cuda_zip_sel, scratch) == offsetof(ZsCall, scratch),
+              "device zip selection layout");
 
 namespace {
 
@@ -668,6 +672,8 @@ int32_t mz_cuda_zip_parse_directory(const void *d_archive, uint64_t len, mz_cuda
         dir->max_clen[k] = h.max_clen[k];
     }
     const bool fits = dir->max_entries >= m && (!dir->decode || dir->out_cap >= h.out); /* otherwise MZ_BUF_ERROR: nothing listed */
+    const bool own = fits && !dir->entries && dir->alloc_entries && m;
+    if (own) CK(cudaMalloc(&dir->entries, (size_t)m * sizeof(ZipDevEnt)));
     const bool pub = fits && dir->entries, dec = fits && dir->decode;
     if (!m || (!pub && !dec)) return MZ_OK;
     /* 5. extents, tables */
@@ -802,6 +808,92 @@ int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t c
     const uint32_t per = ZW_THREADS / 32;
     if (W.n) MZ_LAUNCH(zw_emit_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, cd_off);
     MZ_LAUNCH(zw_end_kernel, dim3(1), dim3(1), 0, s, W, cd_off, cd_size);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+/* ---- K12: random access to an archive in device memory ----------------------------------------------------------- */
+int32_t mz_cuda_zip_name_index(const void *d_archive, const void *d_entries, uint32_t n, uint64_t *d_table, uint32_t P, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (n == 0) return MZ_OK;
+    if (!d_archive || !d_entries || !d_table || P < 2ull * n || (P & (P - 1))) return MZ_PARAM_ERROR;
+    MZ_LAUNCH(zs_index_kernel, dim3((n + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_archive,
+              (const ZipDevEnt *)d_entries, n, (unsigned long long *)d_table, P);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_name_lookup(const void *d_archive, const void *d_entries, const uint64_t *d_table, uint32_t P, const void *d_names,
+                                const uint64_t *d_name_off, const uint32_t *d_name_len, uint32_t nq, uint8_t ignore_case, uint32_t *d_index,
+                                void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (nq == 0) return MZ_OK;
+    if (!d_names || !d_name_off || !d_name_len || !d_index || (P & (P - 1)) || (P && (!d_archive || !d_entries || !d_table))) return MZ_PARAM_ERROR;
+    MZ_LAUNCH(zs_lookup_kernel, dim3((nq + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, (cudaStream_t)stream, (const uint8_t *)d_archive,
+              (const ZipDevEnt *)d_entries, (const unsigned long long *)d_table, P, (const uint8_t *)d_names, d_name_off, d_name_len, nq,
+              (uint32_t)(ignore_case != 0), d_index);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+extern "C++" {
+namespace {
+ZsCall zs_call(const mz_cuda_zip_sel *c) {
+    ZsCall C;
+    memcpy(&C, c, sizeof(C));
+    return C;
+}
+} // namespace
+} // extern "C++"
+
+int32_t mz_cuda_zip_sel_counts(const mz_cuda_zip_sel *sc, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!sc || !sc->cnt || !sc->pre || !sc->part || (sc->n && (!sc->select || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
+    const ZsCall C = zs_call(sc);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (C.n) MZ_LAUNCH(zs_count_kernel, dim3((C.n + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, s, C);
+    CK(cudaGetLastError());
+    return zw_scan<ZsCount>(C.cnt, C.n, C.pre, (ZsCount *)C.part, s);
+}
+
+int32_t mz_cuda_zip_sel_fill(const mz_cuda_zip_sel *sc, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!sc || !sc->pre || (sc->sel && sc->n && (!sc->select || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
+    const ZsCall C = zs_call(sc);
+    MZ_LAUNCH(zs_fill_kernel, dim3(C.n / ZS_THREADS + 1), dim3(ZS_THREADS), 0, (cudaStream_t)stream, C);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_sel_gather(const mz_cuda_zip_sel *sc, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!sc || !sc->pre || (sc->n && (!sc->select || !sc->archive || !sc->scratch || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
+    if (sc->n == 0) return MZ_OK;
+    const uint32_t per = ZS_THREADS / 32, g = (sc->n + per - 1) / per, cap = (uint32_t)c->sm_count * 8u;
+    MZ_LAUNCH(zs_gather_kernel, dim3(g < cap ? g : cap), dim3(ZS_THREADS), 0, (cudaStream_t)stream, zs_call(sc));
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_sel_status(const uint32_t *d_status, const uint32_t *d_select, uint32_t n, uint32_t count, int32_t *d_out, uint64_t *d_first,
+                               void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (n == 0) return MZ_OK;
+    if (!d_status || !d_select || !d_first) return MZ_PARAM_ERROR;
+    MZ_LAUNCH(zs_status_kernel, dim3((n + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, (cudaStream_t)stream, d_status, d_select, n, count,
+              d_out, (unsigned long long *)d_first);
     CK(cudaGetLastError());
     return MZ_OK;
 }

@@ -2112,6 +2112,287 @@ static uint8_t *zw_carve(const size_t *sz, void **out[], int k) {
     return w;
 }
 
+/* ---- random access to an archive in device memory (mz_zip_cuda_reader_*) ------------------------------------------------- */
+struct mz_zip_cuda_dev_reader {
+    int32_t device;
+    uint32_t count, P;                /* accepted entries; slots of the name index (0 when there are no entries) */
+    const uint8_t *archive;
+    uint64_t cd_off, max_clen[4];
+    char *password;
+    mz_cuda_zip_dev_entry *entries;   /* K10: the public table */
+    mz_cuda_zip_ent *ent;             /* K10: the archive-wide K9 table (local header and extent in the archive) */
+    void *sha;                        /* K10: expected digests, the rows sha_slot names */
+    uint64_t *table;                  /* K12: the name index */
+    /* a selection's round, kept between calls and grown when a selection needs more */
+    uint32_t cap;                     /* slots the arrays below hold */
+    uint8_t *work, *selw;             /* zd_carve's arrays; the counts, their scan, the selection's K9 table, the first-failure word */
+    zr_slot z;
+    mz_cuda_zip_sel_count *cnt, *pre;
+    void *part;
+    mz_cuda_zip_ent *sel;
+    uint64_t *first;
+    uint8_t *gbuf;                    /* gathered extents of a selection with WinZip AES entries, 32 zero bytes behind them */
+    uint64_t gcap;
+};
+
+static int32_t zu_enter(const mz_zip_cuda_dev_reader *r, int32_t *prev) {
+    *prev = mz_cuda_get_device();
+    return *prev == r->device ? MZ_OK : mz_cuda_set_device(r->device);
+}
+
+static void zu_leave(const mz_zip_cuda_dev_reader *r, int32_t prev) {
+    if (prev >= 0 && prev != r->device)
+        mz_cuda_set_device(prev);
+}
+
+/* the round arrays for at least n slots (sized to a power of two, at least 256); MZ_OK or MZ_MEM_ERROR */
+static int32_t zu_reserve(mz_zip_cuda_dev_reader *r, uint32_t n) {
+    if (r->work && n <= r->cap)
+        return MZ_OK;
+    uint64_t cap = 256;
+    while (cap < n)
+        cap <<= 1;
+    if (cap > 0xffffffffull)
+        cap = 0xffffffffull;
+    mz_cuda_free(r->work);
+    mz_cuda_free(r->selw);
+    r->work = r->selw = NULL;
+    r->cap = 0;
+    uint32_t *unused;
+    r->z.nsha = 1; /* zd_carve: a digest row per slot */
+    r->work = zd_carve(&r->z, (uint32_t)cap, &unused);
+    const size_t m = (size_t)cap;
+    const size_t sz[5] = {m * sizeof(mz_cuda_zip_sel_count), (m + 1) * sizeof(mz_cuda_zip_sel_count),
+                          (m / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_sel_count), m * sizeof(mz_cuda_zip_ent), 8};
+    void **out[5] = {(void **)&r->cnt, (void **)&r->pre, &r->part, (void **)&r->sel, (void **)&r->first};
+    if (r->work)
+        r->selw = zw_carve(sz, out, 5);
+    if (!r->work || !r->selw) {
+        mz_cuda_free(r->work);
+        r->work = NULL;
+        return MZ_MEM_ERROR;
+    }
+    r->cap = (uint32_t)cap;
+    return MZ_OK;
+}
+
+int32_t mz_zip_cuda_reader_open(const void *d_archive, uint64_t len, const char *password, mz_zip_cuda_dev_reader **reader, uint32_t *count,
+                                int32_t *refuse, mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    if (!reader || !count || !refuse || (!d_archive && len))
+        return MZ_PARAM_ERROR;
+    *reader = NULL;
+    *count = 0;
+    *refuse = MZ_OK;
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    const double t0 = now_ms();
+    mz_cuda_zip_dir dir;
+    memset(&dir, 0, sizeof(dir));
+    dir.have_password = password != NULL;
+    dir.password_long = password && strlen(password) > 128;
+    dir.max_entries = 0xffffffffu;
+    dir.decode = 1;
+    dir.out_cap = ~0ull;
+    dir.alloc_entries = 1; /* the public table, allocated by the parse once it knows the count */
+    int32_t err = mz_cuda_zip_parse_directory(d_archive, len, &dir, stream);
+    if (err == MZ_OK && dir.err)
+        err = dir.err; /* the archive as a whole */
+    st.pack_ms = now_ms() - t0;
+    mz_zip_cuda_dev_reader *r = NULL;
+    if (!err && dir.count > (1u << 30))
+        err = MZ_SUPPORT_ERROR; /* the name index holds 2 x count slots in 32 bits */
+    if (!err && !(r = (mz_zip_cuda_dev_reader *)calloc(1, sizeof(*r))))
+        err = MZ_MEM_ERROR;
+    if (r)
+        r->device = mz_cuda_get_device();
+    if (!err && password && !(r->password = strdup(password)))
+        err = MZ_MEM_ERROR;
+    if (!err) {
+        r->count = dir.count;
+        r->archive = (const uint8_t *)d_archive;
+        r->cd_off = dir.cd_off;
+        memcpy(r->max_clen, dir.max_clen, sizeof(r->max_clen));
+        r->entries = (mz_cuda_zip_dev_entry *)dir.entries;
+        r->ent = dir.ent;
+        r->sha = dir.sha_expect;
+        dir.entries = NULL; /* the reader's now */
+        dir.ent = NULL;
+        dir.sha_expect = NULL;
+        if (r->count) {
+            r->P = 2;
+            while (r->P < 2 * r->count)
+                r->P <<= 1;
+            const double t1 = now_ms();
+            r->table = (uint64_t *)mz_cuda_malloc((size_t)r->P * 8);
+            st.setup_ms = now_ms() - t1;
+            if (!r->table)
+                err = MZ_MEM_ERROR;
+            const double t2 = now_ms();
+            if (!err) err = mz_cuda_memset(r->table, 0xff, (size_t)r->P * 8, stream);
+            if (!err) err = mz_cuda_zip_name_index(d_archive, r->entries, r->count, r->table, r->P, stream);
+            if (!err) err = mz_cuda_stream_sync(stream);
+            st.gpu_ms = now_ms() - t2;
+        }
+    }
+    mz_cuda_free(dir.entries);
+    mz_cuda_free(dir.ent);
+    mz_cuda_free(dir.sha_expect);
+    if (err) {
+        mz_zip_cuda_reader_close(r);
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    st.entries = dir.count;
+    st.bytes_in = dir.bytes_in;
+    st.bytes_out = dir.bytes_out;
+    *reader = r;
+    *count = dir.count;
+    *refuse = dir.refuse;
+    if (stats)
+        *stats = st;
+    return MZ_OK;
+}
+
+const mz_cuda_zip_dev_entry *mz_zip_cuda_reader_entries(const mz_zip_cuda_dev_reader *reader) {
+    return reader ? reader->entries : NULL;
+}
+
+int32_t mz_zip_cuda_reader_locate(mz_zip_cuda_dev_reader *r, const void *d_names, const uint64_t *d_name_off, const uint32_t *d_name_len,
+                                  uint32_t n, uint8_t ignore_case, uint32_t *d_index, void *stream) {
+    if (!r || (n && (!d_names || !d_name_off || !d_name_len || !d_index)))
+        return MZ_PARAM_ERROR;
+    int32_t prev;
+    int32_t err = zu_enter(r, &prev);
+    if (!err) err = mz_cuda_zip_name_lookup(r->archive, r->entries, r->table, r->P, d_names, d_name_off, d_name_len, n, ignore_case, d_index, stream);
+    zu_leave(r, prev);
+    return err;
+}
+
+int32_t mz_zip_cuda_reader_decode(mz_zip_cuda_dev_reader *r, const uint32_t *d_select, uint32_t nsel, void *d_out, uint64_t out_cap,
+                                  uint64_t *out_bytes, uint64_t *d_out_off, int32_t *d_status, mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    if (!r || !out_bytes || (!d_select && nsel) || ((uintptr_t)d_out & 15))
+        return MZ_PARAM_ERROR;
+    *out_bytes = 0;
+    int32_t prev;
+    int32_t err = zu_enter(r, &prev);
+    const double t0 = now_ms();
+    if (!err && !(r->work && nsel <= r->cap)) {
+        err = zu_reserve(r, nsel);
+        st.setup_ms += now_ms() - t0;
+    }
+    /* 1. per-slot counts and their scan; the totals come back */
+    mz_cuda_zip_sel sc;
+    memset(&sc, 0, sizeof(sc));
+    sc.archive = r->archive;
+    sc.ent = r->ent;
+    sc.count = r->count;
+    sc.n = nsel;
+    sc.select = d_select;
+    sc.cnt = r->cnt;
+    sc.pre = r->pre;
+    sc.part = r->part;
+    mz_cuda_zip_sel_count tot;
+    memset(&tot, 0, sizeof(tot));
+    if (!err) err = mz_cuda_zip_sel_counts(&sc, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&tot, r->pre + nsel, sizeof(tot), stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    st.pack_ms = now_ms() - t0 - st.setup_ms;
+    if (!err) {
+        *out_bytes = tot.out;
+        st.entries = nsel;
+        st.bytes_in = tot.cin;
+        st.bytes_out = tot.cout;
+        if (d_out && out_cap < tot.out)
+            err = MZ_BUF_ERROR;
+    }
+    if (err || !d_out || !nsel) { /* sizing call, an empty selection, or an error: at most the offsets */
+        sc.out_off = d_out_off;
+        if (!err && d_out_off) err = mz_cuda_zip_sel_fill(&sc, stream);
+        if (!err) err = mz_cuda_stream_sync(stream);
+        zu_leave(r, prev);
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    /* 2. the selection's K9 table, and with WinZip AES entries every slot's extent gathered into scratch (K8 decrypts in place) */
+    const int gather = tot.a[1] || tot.a[2] || tot.a[3];
+    if (gather && tot.gather + 32 > r->gcap) {
+        const double t1 = now_ms();
+        mz_cuda_free(r->gbuf);
+        r->gcap = 0;
+        if (!(r->gbuf = (uint8_t *)mz_cuda_malloc(tot.gather + 32)))
+            err = MZ_MEM_ERROR;
+        else
+            r->gcap = tot.gather + 32;
+        st.setup_ms += now_ms() - t1;
+    }
+    const double t2 = now_ms();
+    sc.gather = gather;
+    sc.sel = r->sel;
+    sc.out_off = d_out_off;
+    sc.scratch = r->gbuf;
+    if (!err) err = mz_cuda_zip_sel_fill(&sc, stream);
+    if (!err && gather) {
+        err = mz_cuda_memset(r->gbuf + tot.gather, 0, 32, stream);
+        if (!err) err = mz_cuda_zip_sel_gather(&sc, stream);
+    }
+    /* 3. the round (K9 locate, K8, stored copy, K5, K1, K7, K9 verify), then each slot's status and the first failing slot */
+    zr_slot *z = &r->z;
+    z->n = nsel;
+    z->njobs = tot.job;
+    z->nsha = tot.sha;
+    memcpy(z->na, tot.a, sizeof(z->na));
+    z->na[0] = 0;
+    memcpy(z->max_clen, r->max_clen, sizeof(z->max_clen)); /* the archive's largest ciphertext per strength: K8's bound */
+    z->password = r->password;
+    z->d_ent = r->sel;
+    z->d_sha = (uint8_t *)r->sha;
+    /* in place: buf_len = cd_off as extract_device reads it; gathered: the extents, 32 zero bytes behind them */
+    if (!err) err = zr_launch(z, gather ? r->gbuf : (uint8_t *)r->archive, gather ? tot.gather : r->cd_off, (uint8_t *)d_out, stream);
+    if (!err) err = mz_cuda_memset(r->first, 0xff, 8, stream);
+    if (!err) err = mz_cuda_zip_sel_status(z->d_status, d_select, nsel, r->count, d_status, r->first, stream);
+    uint64_t first = ~0ull;
+    if (!err) err = mz_cuda_memcpy_d2h(&first, r->first, 8, stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    if (!err && first != ~0ull)
+        err = -(int32_t)(uint32_t)first;
+    st.gpu_ms = now_ms() - t2;
+    st.rounds = 1;
+    mz_cuda_stream_sync(stream);
+    zu_leave(r, prev);
+    if (stats)
+        *stats = st;
+    return err;
+}
+
+void mz_zip_cuda_reader_close(mz_zip_cuda_dev_reader *r) {
+    if (!r)
+        return;
+    int32_t prev;
+    zu_enter(r, &prev);
+    mz_cuda_free(r->entries);
+    mz_cuda_free(r->ent);
+    mz_cuda_free(r->sha);
+    mz_cuda_free(r->table);
+    mz_cuda_free(r->work);
+    mz_cuda_free(r->selw);
+    mz_cuda_free(r->gbuf);
+    zu_leave(r, prev);
+    free(r->password);
+    free(r);
+}
+
 int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags,
                                  const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
                                  mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream) {
