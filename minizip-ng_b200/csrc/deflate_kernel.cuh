@@ -70,13 +70,17 @@ constexpr int DF_OFF_HIST2 = DF_OFF_HIST + (288 + 32) * 4;   /* u32[256]: second
 constexpr int DF_OFF_CODE = DF_OFF_HIST2 + 256 * 4;          /* u32[288 + 32]: code | len << 16 | extra bits << 20 */
 constexpr int DF_OFF_LENS = DF_OFF_CODE + (288 + 32) * 4;    /* u8[288 + 32] code lengths (header) */
 constexpr int DF_OFF_BITS = DF_OFF_LENS + (288 + 32);        /* u8[288 + 32] code length + extra bits */
-constexpr int DF_OFF_SCAN = DF_OFF_BITS + (288 + 32);        /* u32[256]: [0,128) per (batch, warp) partials, [128,256) scanned */
+constexpr int DF_OFF_SCAN = DF_OFF_BITS + (288 + 32);        /* u32[256]: block-scan scratch */
 constexpr int DF_OFF_BB = DF_OFF_SCAN + 256 * 4;             /* u32[512] code-builder scratch */
 constexpr int DF_OFF_MISC = DF_OFF_BB + 512 * 4;             /* u32[32] + mbarrier */
 constexpr int DF_OFF_SINK = DF_OFF_MISC + 32 * 4 + 16;       /* u32[32]: one word per lane, the target of atomics that have nothing to do
                                                               * (ptxas branches around a predicated ATOMS; a select on the address is one instruction) */
 constexpr int DF_OFF_LSYM = DF_OFF_SINK + 32 * 4;            /* u16[256]: length - 3 -> length symbol (0..28) | extra value << 5; filled once per CTA */
 constexpr int DF_SMEM_BYTES = DF_OFF_LSYM + 256 * 2;
+/* u8[16 warps][256]: during the parse and M0, each warp's list of its spans with a capped match (batch << 5 | lane). It lies on the
+ * histograms, code words, lengths and bits: dead from the emit pass of the unit before until the histograms are cleared after M0. */
+constexpr int DF_OFF_CAPL = DF_OFF_HIST;
+static_assert(DF_OFF_CAPL + DF_WARPS * DF_NBATCH * 32 <= DF_OFF_SCAN, "capped-span lists fit in front of the scan scratch");
 constexpr uint32_t DF_ZERO_SYM = 286;                        /* literal/length symbol that never occurs: its table entries are all zero */
 static_assert(DF_HASH_ENTRIES * 4 <= DF_STAGE_WORDS * 4, "hash fits the staging region");
 /* The history variant (template parameter HIST, levels 6-9): the previous 32 KiB -- the chunk's first unit, or with DF_FLAG_DICT the
@@ -207,10 +211,16 @@ __device__ inline uint32_t block_excl_sum(uint32_t v, uint32_t *scan, uint32_t &
  * column `phase` of the CTA's row of g_df_phases (column DF_PH_UNITS counts the units). After a barrier every thread of the CTA is
  * done with the phase before, so the deltas are the CTA's wall time per phase; no barrier is added. Inside D the same marks split
  * the phase at its named barriers (thread 0 takes part in D) into the DF_PH_D_* columns, whose sum is at most D's; the rest of D
- * is the header. DF_PH_D_PASSES + n counts the units whose Kraft completion ran n passes (the last bucket: 7 or more). Without the
- * macro (the product library) and on the emulator the marks compile to nothing. */
+ * is the header. DF_PH_D_PASSES + n counts the units whose Kraft completion ran n passes (the last bucket: 7 or more). The parse
+ * is split the same way at the two barriers of each batch (DF_PH_P_*: (a) up to the first: loads, hashes, reads of the table as
+ * earlier batches left it; (b) up to the second: the inserts; (c) thread 0's own rest of the batch: reads after the insert,
+ * verification, walk, record stores -- a batch's (a) includes the wait for the other warps' (c) of the batch before). M0 has no
+ * barrier inside: its DF_PH_M_* columns are thread 0's time in the capped-span index, the near-source test and the extension
+ * (whatever is left of M0 is waiting at its closing barrier for the other warps). Without the macro (the product library) and on
+ * the emulator the marks compile to nothing. */
 enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_E_SCAN, DF_PH_F_M3, DF_PH_FLUSH, DF_PH_UNITS,
-       DF_PH_D_STATS, DF_PH_D_SWEEP1, DF_PH_D_SWEEP2, DF_PH_D_KRAFT, DF_PH_D_CANON, DF_PH_D_PASSES, DF_PH_COLS = DF_PH_D_PASSES + 8 };
+       DF_PH_D_STATS, DF_PH_D_SWEEP1, DF_PH_D_SWEEP2, DF_PH_D_KRAFT, DF_PH_D_CANON, DF_PH_D_PASSES,
+       DF_PH_P_A = DF_PH_D_PASSES + 8, DF_PH_P_B, DF_PH_P_C, DF_PH_M_INDEX, DF_PH_M_NEAR, DF_PH_M_EXTEND, DF_PH_COLS };
 constexpr int DF_PH_ROWS = 1024;
 #if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
 __device__ unsigned long long g_df_phases[DF_PH_ROWS][DF_PH_COLS];
@@ -543,6 +553,17 @@ __device__ __forceinline__ uint32_t extend_match8(const Smem &sm, uint32_t c, ui
     return len < maxlen ? len : maxlen;
 }
 
+/* p ? a : b as one SEL: left to itself, ptxas branches around the few instructions that compute a */
+__device__ __forceinline__ uint32_t sel_u32(bool p, uint32_t a, uint32_t b) {
+#ifdef MZ_EMU
+    return p ? a : b;
+#else
+    uint32_t r;
+    asm("{\n.reg .pred q;\nsetp.ne.u32 q, %3, 0;\nselp.b32 %0, %1, %2, q;\n}" : "=r"(r) : "r"(a), "r"(b), "r"((uint32_t)p));
+    return r;
+#endif
+}
+
 /* The constant 4 as a value the compiler cannot see (the kernel always runs DF_THREADS threads per CTA): an address `i * k4 + base`
  * stays one IMAD on the FMA pipe, where `i * 4 + base` would become a LEA on the integer-ALU pipe -- the pipe this kernel is bound
  * by. (A constant behind an inline-asm mov would not do: ptxas folds it.) */
@@ -839,10 +860,12 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
 
             if (P.level != 0) {
                 /* ---- A + W: batches ------------------------------------------------------------------ */
+                DF_PHASE_BEGIN(p_t);
+                uint32_t ncap = 0; /* the warp's capped spans so far (uniform in the warp) */
 #pragma unroll 1
                 for (uint32_t b = 0; b < nb; b++) {
                     const uint32_t q0 = b * DF_BATCH + tid * DF_SPAN;
-                    uint32_t v[12], ha[8], lc[8];
+                    uint32_t v[12], ha[8], lc[8]; /* lc: the key read before the batch's inserts, then the position's match record */
                     const uint32_t k4 = opaque4();
                     {
                         const uint2 x = sm.ld64(DF_OFF_IN + q0), y = sm.ld64(DF_OFF_IN + q0 + 8);
@@ -861,41 +884,47 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     }
                     const uint32_t nvalid = ulen > q0 ? (ulen - q0 < 8 ? ulen - q0 : 8u) : 0u;
                     __syncthreads();
-                    {
-                        const uint32_t key0 = ((uint32_t)(DF_NBATCH - 1 - b) << 16) | (CUR + q0);
-                        /* positions at or behind the end of the unit (zero padding, stale bytes) are inserted as well: they lie behind
-                         * every valid position, so they never win a bucket a valid position of this batch hashes to, are never
-                         * "before" anybody, and no batch follows a short unit -- cheaper than a select per key */
+                    DF_PHASE(p_t, DF_PH_P_A);
+                    const uint32_t key0 = ((uint32_t)(DF_NBATCH - 1 - b) << 16) | (CUR + q0);
+                    /* positions at or behind the end of the unit (zero padding, stale bytes) are inserted as well: they lie behind
+                     * every valid position, so they never win a bucket a valid position of this batch hashes to, are never
+                     * "before" anybody, and no batch follows a short unit -- cheaper than a select per key */
 #pragma unroll
-                        for (int j = 0; j < 8; j++) sm.red_min32(ha[j], key0 + j);
-                    }
+                    for (int j = 0; j < 8; j++) sm.red_min32(ha[j], key0 + j);
                     __syncthreads();
+                    DF_PHASE(p_t, DF_PH_P_B);
+                    /* Verify, and turn each candidate into the position's match record (the span record's form below, 0 for none).
+                     * The choice is made on the keys themselves: this batch's keys are the youngest, and my own insert makes the
+                     * bucket's key at most mine, so a smaller key is an earlier position of this batch with the same hash; else the
+                     * candidate is the key read before the batch (~0: none). Outside the history variant the key's age bits may
+                     * stay in c: only the low five bits of the shift amount count, the address keeps bits 2-15, a present key
+                     * lies before me, and distance - 1 (below 32768) is the low 15 bits of the key difference. */
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
                         if (j % STRIDE != 0) {
                             lc[j] = 0;
                             continue;
                         }
-                        const uint32_t cn = sm.ld32(ha[j]) & 0xffffu;
-                        const uint32_t pq = CUR + q0 + j; /* my position as the keys count it */
-                        const uint32_t c = cn < pq ? cn : (lc[j] & 0xffffu);
-                        const uint32_t ca = DF_OFF_IN - CUR + (c & ~3u);
+                        const uint32_t kp = key0 + j, kn = sm.ld32(ha[j]);
+                        const uint32_t ck = kn < kp ? kn : lc[j];
+                        const uint32_t c = HIST ? ck & 0xffffu : ck;
+                        const uint32_t ca = DF_OFF_IN - CUR + (c & 0xfffcu);
                         const uint32_t w0 = sm.ld32(ca), w1 = sm.ld32(ca + 4), w2 = sm.ld32(ca + 8);
                         const uint32_t s = c << 3;
                         const uint32_t x0 = __funnelshift_r(w0, w1, s) ^ v[j];
                         const uint32_t x1 = __funnelshift_r(w1, w2, s) ^ v[j + 4];
                         /* (history variant: a candidate more than 32768 back is out of DEFLATE's reach) */
-                        const bool reach = c < pq && (!HIST || c >= q0 + j);
-                        const uint32_t l = (reach && x0 == 0) ? 4u + ((uint32_t)__clz((int)__brev(x1)) >> 3) : 0u;
-                        lc[j] = l | ((pq - c - 1u) << 4); /* length | distance - 1 */
+                        const bool reach = HIST ? c < CUR + q0 + j && c >= q0 + j : ck != 0xffffffffu;
+                        /* length - 3 = 1 + the further bytes that agree (0..4); in place at bit 3: that count's bits 3-5 + 8 */
+                        const uint32_t l3 = ((uint32_t)__clz((int)__brev(x1)) & ~7u) + 8u;
+                        lc[j] = sel_u32(reach && x0 == 0, (((kp - ck - 1u) << 11) & (0x7fffu << 11)) + l3 + (uint32_t)j, 0u);
                     }
                     if (q0 + 16 > ulen) { /* unit tail: the zero padding must not be matched */
 #pragma unroll
                         for (int j = 0; j < 8; j += STRIDE) {
                             const uint32_t room = ulen > q0 + j ? ulen - (q0 + j) : 0u;
-                            uint32_t l = lc[j] & 15u;
-                            l = l < room ? l : room;
-                            lc[j] = (lc[j] & ~15u) | (l >= (uint32_t)DF_MINMATCH ? l : 0u);
+                            const uint32_t l = rec_len(lc[j]);
+                            lc[j] = l >= (uint32_t)DF_MINMATCH && l > room ? (room >= (uint32_t)DF_MINMATCH ? lc[j] - ((l - room) << 3) : 0u) : lc[j];
                         }
                     }
                     /* ---- W: walk the span: static and branch-free. A match whose lockstep length is the cap (8) reaches the end of
@@ -907,22 +936,12 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                          * with a match (A: before it, and after its end, every position is a literal until the next even one), and
                          * then the first even position at or behind A's end that has one (B, which runs past the span). The same
                          * tokens as the walk below, as two chains of selects and two masks. */
-                        uint32_t endA = 0, endB = 0;
 #pragma unroll
-                        for (int j = 6; j >= 0; j -= 2) {
-                            const uint32_t l = lc[j] & 15u;
-                            const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
-                            mA = l ? rec : mA;
-                            endA = l ? (uint32_t)j + l : endA;
-                        }
+                        for (int j = 6; j >= 0; j -= 2) mA = lc[j] ? lc[j] : mA;
+                        const uint32_t endA = (mA & 7u) + rec_len(mA);
 #pragma unroll
-                        for (int j = 6; j >= 2; j -= 2) {
-                            const uint32_t l = lc[j] & 15u;
-                            const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
-                            const bool nextm = l != 0 && (uint32_t)j >= endA;
-                            mB = nextm ? rec : mB;
-                            endB = nextm ? (uint32_t)j + l : endB;
-                        }
+                        for (int j = 6; j >= 2; j -= 2) mB = lc[j] && (uint32_t)j >= endA ? lc[j] : mB;
+                        const uint32_t endB = (mB & 7u) + rec_len(mB);
                         /* positions under no match are literals (no match: end = start = 0) */
                         lit = ~(((1u << endA) - (1u << (mA & 7u))) | ((1u << endB) - (1u << (mB & 7u)))) & 0xffu;
                         span_end = mB ? endB : endA;
@@ -931,10 +950,10 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                         for (int j = 0; j < 8; j++) {
                             const bool take = nxt == (uint32_t)j;
                             if (j % STRIDE == 0) {
-                                const uint32_t l = lc[j] & 15u;
-                                bool ism = take && l >= (uint32_t)DF_MINMATCH;
-                                if (LAZY && STRIDE == 1 && j < 7) ism = ism && !((lc[j + 1] & 15u) > l);
-                                const uint32_t rec = (uint32_t)j | ((l - 3) << 3) | ((lc[j] >> 4) << 11);
+                                const uint32_t rec = lc[j], l = rec_len(rec);
+                                bool ism = take && rec != 0;
+                                /* (the length fields compare as the lengths do; 0 = none) */
+                                if (LAZY && STRIDE == 1 && j < 7) ism = ism && !(((lc[j + 1] >> 3) & 255u) > ((rec >> 3) & 255u));
                                 const bool first = mA == 0;
                                 if (ONEM) ism = ism && first;
                                 mA = (ism && first) ? rec : mA;
@@ -952,28 +971,30 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                     lit &= (1u << nvalid) - 1u;
                     {
                         /* a capped match (lockstep length 8) is the span's last token; its true length is found after the batches,
-                         * by the M0 pass, 32 such matches at a time (inline it kept the warp busy for the 8 lanes that have one) */
+                         * by the M0 pass, 32 such matches at a time (inline it kept the warp busy for the 8 lanes that have one):
+                         * the warp appends its capped spans to its list in batch and lane order */
                         const uint32_t last = mB ? mB : mA;
-                        const uint32_t capped = __ballot_sync(MZ_FULL_MASK, ((last >> 3) & 255u) == (uint32_t)(DF_LOCKLEN - 3));
-                        if (lane == 0) s_scan[b * DF_WARPS + warp] = capped;
+                        const bool cap = ((last >> 3) & 255u) == (uint32_t)(DF_LOCKLEN - 3);
+                        const uint32_t capped = __ballot_sync(MZ_FULL_MASK, cap);
+                        sm.st8_if(cap, DF_OFF_CAPL + warp * 256u + ncap + (uint32_t)__popc(capped & ((1u << lane) - 1u)), (b << 5) | lane);
+                        ncap += (uint32_t)__popc(capped);
                         sm.st64(DF_OFF_REC + (b * DF_THREADS + tid) * 8, mA | ((lit & 63u) << 26), mB | ((lit >> 6) << 26));
                         /* start offset and end (relative to the span) of the span's last match (0 for none) */
                         sm.st16(DF_OFF_SPN + (b * DF_THREADS + tid) * 2, ((last & 7u) << 9) | span_end);
                     }
+                    DF_PHASE(p_t, DF_PH_P_C);
                 }
                 DF_PHASE(ph_t, DF_PH_PARSE); /* (no barrier behind the last batch: warp 0's view; the walks left are uniform work) */
                 /* ---- M0: true lengths of the capped matches ----------------------------------------------------------------- */
                 {
+                    DF_PHASE_BEGIN(m_t);
                     __syncwarp();
-                    uint32_t bmX[DF_NBATCH], totX = 0;
-#pragma unroll
-                    for (int b = 0; b < DF_NBATCH; b++) {
-                        bmX[b] = (uint32_t)b < nb ? s_scan[b * DF_WARPS + warp] : 0u;
-                        totX += (uint32_t)__popc(bmX[b]);
-                    }
-                    for (uint32_t k0 = 0; k0 < totX; k0 += 32) {
-                        const uint32_t sidx = nth_parked(bmX, k0 + lane, warp);
-                        if (sidx != 0xffffffffu) {
+                    for (uint32_t k0 = 0; k0 < ncap; k0 += 32) {
+                        const uint32_t k = k0 + lane;
+                        const uint32_t e = k < ncap ? sm.ld8(DF_OFF_CAPL + warp * 256u + k) : 0u;
+                        const uint32_t sidx = (e >> 5) * (uint32_t)DF_THREADS + warp * 32u + (e & 31u);
+                        DF_PHASE(m_t, DF_PH_M_INDEX);
+                        if (k < ncap) {
                             const uint2 r = sm.ld64(DF_OFF_REC + sidx * 8);
                             const bool second = (r.y & 0x03ffffffu) != 0;
                             const uint32_t w = second ? r.y : r.x, last = w & 0x03ffffffu;
@@ -1020,6 +1041,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                                     }
                                 }
                             }
+                            DF_PHASE(m_t, DF_PH_M_NEAR);
                             if (l < 64u && l < maxlen) { /* (a near source that runs this far is good enough: skip the second walk) */
                                 const uint32_t lf = extend_match8(sm, c, q, maxlen);
                                 if (lf > l) {
@@ -1029,6 +1051,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                             }
                             sm.st32(DF_OFF_REC + sidx * 8 + (second ? 4u : 0u), (w & ~((255u << 3) | (0x7fffu << 11))) | ((l - 3) << 3) | ((q - cb - 1u) << 11));
                             sm.st16(DF_OFF_SPN + sidx * 2, (j << 9) | (j + l));
+                            DF_PHASE(m_t, DF_PH_M_EXTEND);
                         }
                     }
                 }

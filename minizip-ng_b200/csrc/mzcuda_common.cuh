@@ -77,6 +77,12 @@ struct Smem {
         if (v < *q) *q = v;
     }
     __device__ __forceinline__ void st16_if(bool c, uint32_t off, uint32_t v) const { if (c) st16(off, v); }
+    __device__ __forceinline__ void st8_if(bool c, uint32_t off, uint32_t v) const {
+        if (!c) return;
+        const uint8_t h = (uint8_t)v;
+        MZ_EMU_ACCESS(p(off), 1, EMU_ACC_WRITE, &h);
+        *p(off) = h;
+    }
     __device__ __forceinline__ void red_add32_if(bool c, uint32_t off, uint32_t v) const { if (c) red_add32(off, v); }
     __device__ __forceinline__ void red_or32_if(bool c, uint32_t off, uint32_t v) const { if (c) red_or32(off, v); }
     __device__ __forceinline__ uint2 ld64(uint32_t off) const { MZ_EMU_ACCESS(p(off), 8, EMU_ACC_READ, nullptr); return *(const uint2 *)p(off); }
@@ -125,6 +131,9 @@ struct Smem {
     /* predicated forms: one instruction under a predicate instead of a branch around an asm statement */
     __device__ __forceinline__ void st16_if(bool p, uint32_t off, uint32_t v) const {
         asm volatile("{\n.reg .pred q;\nsetp.ne.u32 q, %2, 0;\n@q st.shared.u16 [%0], %1;\n}" ::"r"(b + off), "r"(v), "r"((uint32_t)p) : "memory");
+    }
+    __device__ __forceinline__ void st8_if(bool p, uint32_t off, uint32_t v) const {
+        asm volatile("{\n.reg .pred q;\nsetp.ne.u32 q, %2, 0;\n@q st.shared.u8 [%0], %1;\n}" ::"r"(b + off), "r"(v), "r"((uint32_t)p) : "memory");
     }
     __device__ __forceinline__ void red_add32_if(bool p, uint32_t off, uint32_t v) const {
         asm volatile("{\n.reg .pred q;\nsetp.ne.u32 q, %2, 0;\n@q red.shared.add.u32 [%0], %1;\n}" ::"r"(b + off), "r"(v), "r"((uint32_t)p) : "memory");

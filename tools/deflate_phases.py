@@ -3,7 +3,10 @@
 libmz_strm_cuda_phases.so, built by `make -C minizip-ng_b200/csrc phases`: deflate_kernel.cuh with -DMZ_DF_PHASES) on the bench
 text with the C5 launch (64 KiB chunks, one launch over the whole buffer, 2 CTAs per SM) and prints SM cycles per 32 KiB unit
 and each phase's share, with the GPU's name, power limit and SM clock. D (the code construction) is split further at its named
-barriers: stats, the two sweeps, Kraft completion (with the number of units per pass count), canonical codes, and the header.
+barriers: stats, the two sweeps, Kraft completion (with the number of units per pass count), canonical codes, and the header. The
+parse is split at the two barriers of each batch: (a) loads, hashes and the reads of the table before the batch's inserts, (b) the
+inserts, (c) thread 0's reads after the inserts, verification, walk and record stores. M0 is split into thread 0's time in the
+capped-span index, the near-source test and the extension; the rest of M0 is the wait for the other warps.
 
 The counters are thread 0's clock64() readings at the kernel's barriers, summed per CTA; cycles per unit = all CTAs' cycles over
 all units. The counting itself costs a few atomics per unit, so the kernel time printed here is not the product's.
@@ -23,7 +26,12 @@ UNITS = len(PHASES)  # column layout of g_df_phases (deflate_kernel.cuh): the ph
 D_SUB = ["stats", "sweep 1", "sweep 2", "Kraft completion", "canonical codes"]  # + "header": the rest of D
 D_COL = PHASES.index("D (codes + header)")
 NPASS = 8  # units whose Kraft completion ran 0, 1, .. 6, 7 or more passes
-COLS = UNITS + 1 + len(D_SUB) + NPASS
+P_SUB = ["(a) loads, hashes, old keys", "(b) inserts", "(c) verify, walk, stores"]  # + "rest": the end of the last batch
+P_COL = PHASES.index("parse batches")
+M_SUB = ["index", "near-source test", "extension"]  # + "wait": the closing barrier
+M_COL = PHASES.index("M0")
+SUB0 = UNITS + 1 + len(D_SUB) + NPASS
+COLS = SUB0 + len(P_SUB) + len(M_SUB)
 ROWS = 1024
 
 
@@ -92,6 +100,10 @@ def main():
     busiest = max(sum(r[:UNITS]) for r in tab) / args.reps
     dsub = [sum(r[UNITS + 1 + i] for r in tab) for i in range(len(D_SUB))]
     dsub.append(per[D_COL] - sum(dsub))
+    psub = [sum(r[SUB0 + i] for r in tab) for i in range(len(P_SUB))]
+    psub.append(per[P_COL] - sum(psub))
+    msub = [sum(r[SUB0 + len(P_SUB) + i] for r in tab) for i in range(len(M_SUB))]
+    msub.append(per[M_COL] - sum(msub))
     passes = [sum(r[UNITS + 1 + len(D_SUB) + i] for r in tab) // args.reps for i in range(NPASS)]  # a CTA's cycles over the launch ~ kernel time x SM clock
     res = {"gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock_after": info.get("clocks.sm"),
            "sm_clock_max": info.get("clocks.max.sm"), "level": args.level, "bytes": n, "ctas": len(tab), "units": units // args.reps,
@@ -100,18 +112,24 @@ def main():
            "phases": {p: {"cycles_per_unit": round(c / units, 0), "share": round(c / total, 4)} for p, c in zip(PHASES, per)},
            "d_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_d": round(c / max(per[D_COL], 1), 4)}
                            for p, c in zip(D_SUB + ["header"], dsub)},
+           "parse_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_parse": round(c / max(per[P_COL], 1), 4)}
+                               for p, c in zip(P_SUB + ["rest"], psub)},
+           "m0_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_m0": round(c / max(per[M_COL], 1), 4)}
+                            for p, c in zip(M_SUB + ["wait"], msub)},
            "kraft_passes": {("%d+" % i if i == NPASS - 1 else str(i)): n for i, n in enumerate(passes)}}
     print("%s, power limit %s, SM clock %s (max %s); effective clock during the launches %d MHz" % (
         res["gpu"], res["power_limit"], res["sm_clock_after"], res["sm_clock_max"], res["effective_sm_MHz"]))
     print("level %d, %.2f GiB of bench text, 64 KiB chunks, %d CTAs, %d units: %.3f ms per launch (instrumented), ratio %.4f" % (
         args.level, n / (1 << 30), res["ctas"], res["units"], kms, res["ratio"]))
-    print("%-20s %12s %7s" % ("phase", "cycles/unit", "share"))
+    print("%-30s %12s %7s" % ("phase", "cycles/unit", "share"))
     for p, c in zip(PHASES, per):
-        print("%-20s %12.0f %6.1f%%" % (p, c / units, 100.0 * c / total))
-        if p == PHASES[D_COL]:
-            for q, d in zip(D_SUB + ["header"], dsub):
-                print("  %-18s %12.0f %6.1f%% of D" % (q, d / units, 100.0 * d / max(per[D_COL], 1)))
-    print("%-20s %12.0f" % ("total", total / units))
+        print("%-30s %12.0f %6.1f%%" % (p, c / units, 100.0 * c / total))
+        for col, names, sub, tag in ((D_COL, D_SUB + ["header"], dsub, "D"), (P_COL, P_SUB + ["rest"], psub, "parse"),
+                                     (M_COL, M_SUB + ["wait"], msub, "M0")):
+            if p == PHASES[col]:
+                for q, d in zip(names, sub):
+                    print("  %-28s %12.0f %6.1f%% of %s" % (q, d / units, 100.0 * d / max(per[col], 1), tag))
+    print("%-30s %12.0f" % ("total", total / units))
     print("units by Kraft completion passes: " + ", ".join("%s: %d" % kv for kv in res["kraft_passes"].items()))
     print(json.dumps(res))
     if args.json:
