@@ -25,8 +25,10 @@
  *              entry per code word: literal byte | length symbol + extra | distance), placed by a block
  *              scan; literal / length / distance histograms by shared-memory atomics on the way
  *   D codes    block-parallel length-limited prefix codes (10 warps, named barrier)
- *   E count    every thread owns an equal, contiguous run of entries: bit totals -> block scan
- *   F emit     every thread packs its run at its bit offset into the staging buffer (aliases the hash table)
+ *   E+F emit   two batches at a time, every thread looks up its two spans' code words, which give the spans' sizes; one warp
+ *              scan of both + one barrier + the pair's 16 warp totals place every span, which then packs its bits at that offset
+ *              into the staging buffer (aliases the hash table). The block's total comes from the histograms in D, so whether
+ *              the block is stored is known before this pass
  *   G flush    staging -> global in 16-byte units; partial tail carried into the next block
  * Blocks that would not shrink are emitted as stored blocks. A unit with more entries than the list
  * holds is coded as two blocks (batch halves). A non-final chunk ends with an empty stored block
@@ -63,7 +65,7 @@ constexpr int DF_OFF_IN = 0;
 constexpr int DF_OFF_HASH = DF_OFF_IN + DF_UNIT + 64;
 constexpr int DF_OFF_STAGE = DF_OFF_HASH;       /* bit staging aliases the hash table (dead after the parse) */
 constexpr int DF_OFF_REC = DF_OFF_HASH + DF_STAGE_WORDS * 4; /* span records: 4096 x 2 words */
-constexpr int DF_OFF_SPN = DF_OFF_REC + DF_NBATCH * DF_THREADS * 8; /* u16 per span: match extent -> cover -> bits -> bit offset */
+constexpr int DF_OFF_SPN = DF_OFF_REC + DF_NBATCH * DF_THREADS * 8; /* u16 per span: match extent -> cover */
 constexpr int DF_SPAN_BYTES = DF_NBATCH * DF_THREADS * 10;
 constexpr int DF_OFF_HIST = DF_OFF_REC + DF_SPAN_BYTES;      /* u32[288 + 32] */
 constexpr int DF_OFF_HIST2 = DF_OFF_HIST + (288 + 32) * 4;   /* u32[256]: second copy of the literal counts (odd lanes) */
@@ -156,7 +158,7 @@ __device__ __forceinline__ void stage_put(uint32_t *stage, uint32_t pos, uint32_
     if (s + n > 32) atomicOr(&stage[w + 1], v >> (32 - s));
 }
 
-/* OR n (<= 15) bits of v into the staging bit string at bit position pos (explicit shared-space form) */
+/* OR n (<= 32) bits of v into the staging bit string at bit position pos (explicit shared-space form) */
 __device__ __forceinline__ void stage_or(const Smem &sm, uint32_t pos, uint32_t v, uint32_t n) {
     const uint32_t sh = pos & 31u, wa = DF_OFF_STAGE + ((pos >> 5) << 2);
     sm.red_or32(wa, v << sh);
@@ -187,25 +189,6 @@ struct BitWriter {
     }
 };
 
-/* block-wide exclusive sum over one value per thread; `scan` = 64 words of shared scratch.
- * Contains __syncthreads: every thread of the CTA must call. */
-__device__ inline uint32_t block_excl_sum(uint32_t v, uint32_t *scan, uint32_t &total) {
-    uint32_t incl = warp_incl_sum(v);
-    if (lane_id() == 31) scan[warp_id()] = incl;
-    __syncthreads();
-    if (warp_id() == 0) {
-        uint32_t w = lane_id() < (unsigned)DF_WARPS ? scan[lane_id()] : 0u;
-        uint32_t wi = warp_incl_sum(w);
-        scan[32 + lane_id()] = wi - w;
-        if (lane_id() == 31) scan[31] = wi; /* grand total parked in slot 31 after use */
-    }
-    __syncthreads();
-    uint32_t res = scan[32 + warp_id()] + incl - v;
-    total = scan[31];
-    __syncthreads();
-    return res;
-}
-
 /* ---- opt-in per-phase cycle counters (compile with -DMZ_DF_PHASES: `make phases`, read by tools/deflate_phases.py) ---------------
  * Thread 0 of every CTA reads clock64() right after the barrier that ends a phase and adds the cycles since its previous reading to
  * column `phase` of the CTA's row of g_df_phases (column DF_PH_UNITS counts the units). After a barrier every thread of the CTA is
@@ -216,11 +199,14 @@ __device__ inline uint32_t block_excl_sum(uint32_t v, uint32_t *scan, uint32_t &
  * earlier batches left it; (b) up to the second: the inserts; (c) thread 0's own rest of the batch: reads after the insert,
  * verification, walk, record stores -- a batch's (a) includes the wait for the other warps' (c) of the batch before). M0 has no
  * barrier inside: its DF_PH_M_* columns are thread 0's time in the capped-span index, the near-source test and the extension
- * (whatever is left of M0 is waiting at its closing barrier for the other warps). Without the macro (the product library) and on
- * the emulator the marks compile to nothing. */
-enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_E_SCAN, DF_PH_F_M3, DF_PH_FLUSH, DF_PH_UNITS,
+ * (whatever is left of M0 is waiting at its closing barrier for the other warps). The count-and-emit pass is split at its barrier
+ * per pair of batches (DF_PH_X_*: (i) up to the barrier: the spans' code words, sizes and the warp scan -- a pair's (i) includes
+ * the wait for the other warps' (ii) of the pair before; (ii) thread 0's own emit of the pair; (iii) M3). Without the macro (the product
+ * library) and on the emulator the marks compile to nothing. */
+enum { DF_PH_LOAD, DF_PH_PARSE, DF_PH_M0, DF_PH_COVER, DF_PH_T_M1, DF_PH_D, DF_PH_EMIT, DF_PH_FLUSH, DF_PH_UNITS,
        DF_PH_D_STATS, DF_PH_D_SWEEP1, DF_PH_D_SWEEP2, DF_PH_D_KRAFT, DF_PH_D_CANON, DF_PH_D_PASSES,
-       DF_PH_P_A = DF_PH_D_PASSES + 8, DF_PH_P_B, DF_PH_P_C, DF_PH_M_INDEX, DF_PH_M_NEAR, DF_PH_M_EXTEND, DF_PH_COLS };
+       DF_PH_P_A = DF_PH_D_PASSES + 8, DF_PH_P_B, DF_PH_P_C, DF_PH_M_INDEX, DF_PH_M_NEAR, DF_PH_M_EXTEND, DF_PH_X_SCAN, DF_PH_X_EMIT,
+       DF_PH_X_M3, DF_PH_COLS };
 constexpr int DF_PH_ROWS = 1024;
 #if defined(MZ_DF_PHASES) && !defined(MZ_EMU)
 __device__ unsigned long long g_df_phases[DF_PH_ROWS][DF_PH_COLS];
@@ -254,7 +240,8 @@ constexpr int DF_BB_THREADS = 320;
 enum { BB_STAT = 0 /* [2][4]: used,total,first */, BB_KRAFT = 8 /* [2 sweeps][2 alph][16] */, BB_SLACK = 136 /* [2] */,
        BB_CNTW = 144 /* [2 bufs][10 warps][16]: codes per length in a warp, then what a code's rank in its warp is set against */,
        BB_NZ = 464 /* [10] ballots: length != 0 */, BB_ST = 474 /* [10] ballots: a run of equal lengths starts here */,
-       BB_HSUM = 484 /* [10] header bits per warp */, BB_HDRBITS = 494 /* size of the block header in bits */ };
+       BB_HSUM = 484 /* [10] header bits per warp */, BB_HDRBITS = 494 /* size of the block header in bits */,
+       BB_TOKBITS = 495 /* bits of the block's code words and extra bits, end of block left out */, BB_TOKW = 496 /* [10] the same per warp */ };
 
 /* ---- block header (RFC 1951 3.2.7): HLIT/HDIST trimmed, code lengths run-length coded (symbols 16/17/18) under a STATIC
  * code-length code. A code chosen per block would save another 0.01-0.09 % of the input (tools/sim/lzsim hdr=0 vs hdr=3) and cost
@@ -465,16 +452,24 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
             const uint32_t code = cntw[w * 16 + L] + (uint32_t)__popc(m & ((1u << lane) - 1));
             cw = (__brev(code) >> (32 - L)) | (L << 16);
         }
+        /* The block's token bits: count x (code length + extra bits) over both alphabets, end of block left out. The histograms
+         * count exactly the symbols the emit pass writes, so this is the sum of the span sizes there. (The counts are read again:
+         * c may hold a count forced to 1 above.) */
+        uint32_t tb;
         if (a == 0) {
             const uint32_t eb = sym >= 257 ? len_extra_bits(sym - 257) : 0u;
             lens_ll[sym] = (uint8_t)L; /* sym up to 287: entries 286, 287 get 0 */
             code_ll[sym] = cw | (eb << 20);
             bits_ll[sym] = (uint8_t)(L + eb);
+            tb = sym == 256 ? 0u : (hist_ll[sym] + (sym < 256 ? hist_lit2[sym] : 0u)) * (L + eb); /* (286, 287: count 0) */
         } else {
             lens_d[sym] = (uint8_t)L;  /* sym up to 31 */
             code_d[sym] = cw;          /* distance extra bits come from the entry, not the table */
             bits_d[sym] = (uint8_t)(L + dist_extra_bits(sym));
+            tb = hist_d[sym] * (L + dist_extra_bits(sym)); /* (30, 31: count 0) */
         }
+        tb = __reduce_add_sync(MZ_FULL_MASK, tb);
+        if (lane == 0) bb[BB_TOKW + w] = tb;
     }
     /* ---- the block header, written straight into the (clean) staging buffer at bit hdrpos. One thread per code length;
      * runs of equal lengths are found from per-warp ballots (a run never crosses from the literal/length lengths into the
@@ -533,6 +528,9 @@ __device__ inline void block_build_codes(const uint32_t *hist_ll, const uint32_t
     if (tid == 0) {
         stage_put(stage, hdrpos, bfinal | (2u << 1) | ((hlit - 257u) << 3) | ((hdist - 1u) << 8) | (15u << 13), 17);
         bb[BB_HDRBITS] = 17 + 57 + total;
+        uint32_t tok = 0;
+        for (uint32_t ww = 0; ww < 10; ww++) tok += bb[BB_TOKW + ww];
+        bb[BB_TOKBITS] = tok;
     }
     if (tid == 32) stage_put(stage, hdrpos + 17, (uint32_t)CL_ORDER57, 32);
     if (tid == 64) stage_put(stage, hdrpos + 17 + 32, (uint32_t)(CL_ORDER57 >> 32), 25);
@@ -678,6 +676,81 @@ __device__ __forceinline__ uint32_t nth_parked(const uint32_t (&bm)[DF_NBATCH], 
         base += up ? (uint32_t)st : 0u;
     }
     return found ? bsel * (uint32_t)DF_THREADS + warp * 32u + base : 0xffffffffu;
+}
+
+/* The count-and-emit pass, first half: a span's code words looked up once (a position that is not a literal looks up the
+ * all-zero entry: no selects on the results). Their lengths, packed one per byte, and the sizes of the span's matches (added
+ * to the byte of the slot they are ordered at) give every bit offset in the span by ONE multiplication per word: byte k of
+ * w * 0x01010101 is the sum of bytes 0..k of w (no byte overflows: 8 x 15 + 2 x 48 < 256), and the top byte of P1 is the sum
+ * of all eight. Kept for the write, no more: the four literal pairs packed for one OR each (at most the two literals of a pair
+ * are in-band, and then they are adjacent: a match start covers its neighbour), the offsets of the slots (E0, E1: byte k = bits
+ * before slot k), the 1 or 2 leftover bytes' code words (xv; they come first) with their bit count and both matches' offsets
+ * (offs), the first match, the span's size (<= 30 + 216 bits; 0 only for a span that holds nothing). */
+struct SpanBits {
+    uint32_t v[4], E0, E1, offs, xv, MA, size;
+};
+template <bool ONEM>
+__device__ __forceinline__ SpanBits span_bits(const Smem &sm, uint32_t sidx, uint32_t F, uint32_t MA, uint32_t MB, uint32_t code_base, uint32_t zero_ent,
+                                              uint32_t k4) {
+    SpanBits s;
+    const uint2 x = sm.ld64(DF_OFF_IN + sidx * DF_SPAN);
+    uint32_t xn = 0;
+    s.xv = 0;
+    const uint32_t ex = (F >> 8) & 3u;
+    if (ex) {
+        const uint32_t c0 = sm.ld32(DF_OFF_CODE + ((F >> 16) & 0xffu) * 4);
+        s.xv = c0 & 0x7fffu;
+        xn = (c0 >> 16) & 15u;
+        if (ex == 2) {
+            const uint32_t c1 = sm.ld32(DF_OFF_CODE + (F >> 24) * 4);
+            s.xv |= (c1 & 0x7fffu) << xn;
+            xn += (c1 >> 16) & 15u;
+        }
+    }
+    uint32_t cw[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const uint32_t by = MZ_BYTE(j < 4 ? x.x : x.y, j & 3);
+        cw[j] = sm.ld32_a(((F >> j) & 1u) ? by * k4 + code_base : zero_ent); /* code | length << 16 (a literal's entry has no extra-bits field) */
+    }
+    /* lengths, one per byte; a match leaves a gap of its size at its slot (slot 8 = none: the shifts clamp to 0) */
+    const uint32_t nA = match_bits(sm, MA), nB = ONEM ? 0u : match_bits(sm, MB);
+    const uint32_t sA = MA ? ((MA >> 28) & 7u) * 8u : 64u, sB = MB ? ((MB >> 28) & 7u) * 8u : 64u;
+    const uint32_t L0 = __byte_perm(__byte_perm(cw[0], cw[1], 0x0062u), __byte_perm(cw[2], cw[3], 0x0062u), 0x5410u) + shl_clamp(nA, sA) + shl_clamp(nB, sB);
+    const uint32_t L1 = __byte_perm(__byte_perm(cw[4], cw[5], 0x0062u), __byte_perm(cw[6], cw[7], 0x0062u), 0x5410u) + shl_clamp(nA, sA - 32u) + shl_clamp(nB, sB - 32u);
+    const uint32_t P0 = L0 * 0x01010101u;                       /* inclusive sums of slots 0..3 */
+    const uint32_t P1 = L1 * 0x01010101u + (P0 >> 24) * 0x01010101u;
+    s.E0 = P0 << 8;
+    s.E1 = __funnelshift_l(P0, P1, 8); /* exclusive: bits before slot k in byte k */
+#pragma unroll
+    for (int jj = 0; jj < 4; jj++) {
+        const uint32_t c0 = cw[2 * jj], c1 = cw[2 * jj + 1];
+        s.v[jj] = (c0 & 0xffffu) | ((c1 & 0xffffu) << (c0 >> 16));
+    }
+    /* the leftover bytes' bits | the first match's offset << 8 | the second's << 16 (each < 256) */
+    s.offs = xn + (((shr_clamp(s.E0, sA) & 0xffu) + (shr_clamp(s.E1, sA - 32u) & 0xffu)) << 8) +
+             (((shr_clamp(s.E0, sB) & 0xffu) + (shr_clamp(s.E1, sB - 32u) & 0xffu)) << 16);
+    s.MA = MA;
+    s.size = xn + (P1 >> 24);
+    return s;
+}
+/* ... second half: the span's bits at bit position pos of the staging buffer. Two literals go out per OR of <= 30 bits; both
+ * target words unconditionally (an OR of zero is cheaper than the branches around it). The first match is OR-ed in here, the
+ * second one's position is parked next to its record (span sidx) for the M3 pass. */
+template <bool ONEM>
+__device__ __forceinline__ void span_emit(const Smem &sm, const SpanBits &s, uint32_t pos, uint32_t sidx, uint32_t stage_base, uint32_t k4) {
+    const uint32_t xn = s.offs & 0xffu;
+    if (xn) stage_or(sm, pos, s.xv, xn);
+    pos += xn;
+#pragma unroll
+    for (int jj = 0; jj < 4; jj++) {
+        const uint32_t pp = pos + MZ_BYTE(jj < 2 ? s.E0 : s.E1, 2 * (jj & 1));
+        const uint32_t wa = stage_word(stage_base, pp, k4);
+        sm.red_or32_a(wa, __funnelshift_l(0u, s.v[jj], pp));
+        sm.red_or32_a(wa + 4, __funnelshift_l(s.v[jj], 0u, pp));
+    }
+    if (s.MA) put_match_bits(sm, pos + ((s.offs >> 8) & 0xffu), s.MA);
+    if (!ONEM) sm.st32(DF_OFF_REC + sidx * 8, pos + (s.offs >> 16)); /* (only read back where MB != 0) */
 }
 
 /* ---- the kernel ------------------------------------------------------------------------------- */
@@ -856,7 +929,6 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
             uint32_t fF[DF_NBATCH], fA[DF_NBATCH];
             bool stored = (P.level == 0);
             const uint32_t bfinal = (last_unit && (flags & DF_FLAG_FINAL)) ? 1u : 0u;
-            uint32_t tokbits = 0;
 
             if (P.level != 0) {
                 /* ---- A + W: batches ------------------------------------------------------------------ */
@@ -1065,8 +1137,8 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 }
                 for (uint32_t i = tid; i < 288 + 32 + 256; i += DF_THREADS) s_hist_ll[i] = 0; /* + the second literal copy */
 
-                /* ---- B: cover. For this pass (and the offset pass below) thread T owns the 8 CONSECUTIVE spans 8T..8T+7 (64
-                 * positions), so one block scan per pass is enough; everything else keeps the parse mapping (span b*512+t),
+                /* ---- B: cover. For this pass thread T owns the 8 CONSECUTIVE spans 8T..8T+7 (64 positions), so one block
+                 * scan is enough; everything else keeps the parse mapping (span b*512+t),
                  * whose shared-memory accesses are conflict-free. cover(span) = the largest end of a match of an earlier
                  * span. Runs: inside a long repeat every span holds a maximal match, and the plain rule would cut each of
                  * them down to the 8 bytes it adds to the cover. A span that lies wholly under the cover and whose match
@@ -1186,48 +1258,7 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                                       s_stage, bitpos, bfinal);
                 __syncthreads(); /* S5 */
                 DF_PHASE(ph_t, DF_PH_D);
-                const uint32_t hdrbits = s_bb[BB_HDRBITS]; /* (the scratch is reused below) */
-                /* ---- E: bits per span -> offsets ------------------------------------------------------------------- */
-                const uint32_t bits_base = sm.addr(DF_OFF_BITS), zero_bits = sm.addr(DF_OFF_BITS + DF_ZERO_SYM);
-#pragma unroll
-                for (int b = 0; b < DF_NBATCH; b++) {
-                    if ((uint32_t)b < nb) {
-                        const uint32_t sidx = (uint32_t)b * DF_THREADS + tid;
-                        const uint32_t F = fF[b];
-                        const uint2 x = sm.ld64(DF_OFF_IN + sidx * DF_SPAN);
-                        uint32_t nbits = match_bits(sm, fA[b]) + (ONEM ? 0u : match_bits(sm, sm.ld32(DF_OFF_REC + sidx * 8 + 4)));
-                        const uint32_t ex = (F >> 8) & 3u;
-                        nbits += ex >= 1 ? sm.ld8(DF_OFF_BITS + ((F >> 16) & 0xffu)) : 0u;
-                        nbits += ex == 2 ? sm.ld8(DF_OFF_BITS + (F >> 24)) : 0u;
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            /* a position that is not a literal reads the all-zero entry (like the emit pass: a select on the address, no
-                             * select on the value) */
-                            nbits += sm.ld8_a(((F >> j) & 1u) ? bits_base + MZ_BYTE(j < 4 ? x.x : x.y, j & 3) : zero_bits);
-                        }
-                        sm.st16(DF_OFF_SPN + sidx * 2, nbits);
-                    }
-                }
-                __syncthreads(); /* S6 */
-                {
-                    uint32_t c[8];
-                    if (tid * 8 < nb * DF_THREADS) {
-                        const uint4 q = *(const uint4 *)(smem + DF_OFF_SPN + tid * 16);
-                        c[0] = q.x & 0xffffu; c[1] = q.x >> 16; c[2] = q.y & 0xffffu; c[3] = q.y >> 16;
-                        c[4] = q.z & 0xffffu; c[5] = q.z >> 16; c[6] = q.w & 0xffffu; c[7] = q.w >> 16;
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < 8; k++) c[k] = 0;
-                    }
-                    uint32_t r[8], acc = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) { r[k] = acc; acc += c[k]; }
-                    const uint32_t mybase = block_excl_sum(acc, s_scan, tokbits); /* S7, S8 inside */
-                    *(uint4 *)(smem + DF_OFF_SPN + tid * 16) = make_uint4(r[0] | (r[1] << 16), r[2] | (r[3] << 16), r[4] | (r[5] << 16), r[6] | (r[7] << 16));
-                    s_bb[tid] = mybase;
-                }
-                __syncthreads(); /* S9: offsets visible */
-                DF_PHASE(ph_t, DF_PH_E_SCAN);
+                const uint32_t hdrbits = s_bb[BB_HDRBITS], tokbits = s_bb[BB_TOKBITS];
                 const uint32_t eob = s_code_ll[256];
                 const uint32_t dyn_bits = hdrbits + tokbits + ((eob >> 16) & 15u);
                 const uint32_t stored_bits = (((bitpos + 3 + 7) & ~7u) - bitpos) + 32 + ulen * 8;
@@ -1239,63 +1270,48 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                         s_stage[w0 + i] = i == 0 ? s_stage[w0] & ((1u << (bitpos & 31u)) - 1u) : 0u;
                     __syncthreads();
                 } else {
-                    /* ---- F: emit. The eight code words of a span are looked up first (a position that is not a literal looks
-                     * up the all-zero entry: no selects on the results); their lengths, packed one per byte, and the sizes of the
-                     * span's matches (added to the byte of the slot they are ordered at) give every bit offset of the span by
-                     * ONE multiplication per word: byte k of w * 0x01010101 is the sum of bytes 0..k of w (no byte overflows:
-                     * 8 x 15 + 2 x 48 < 256). Two literals go out per OR of <= 30 bits; both target words unconditionally (an OR
-                     * of zero is cheaper than the branches around it). The first match is OR-ed in by its span, the second
-                     * one's position is parked next to its record for the M3 pass. ------------------------------------------- */
-                    const uint32_t base = bitpos + hdrbits;
+                    /* ---- E + F: count and emit, two batches at a time. span_bits() looks up a span's code words once and gives
+                     * its size and every bit offset inside it. One warp scan covers both batches (the sizes packed in 16-bit
+                     * halves: a warp's total per batch is at most 32 x 246 bits), the warp totals go to s_scan (one slot per batch
+                     * pair and warp, never rewritten in a unit), and one barrier per pair places every span: spans of a batch are
+                     * in stream order by thread, the second batch follows the first, and each pair starts where the one before
+                     * ended (`run`). The spans are then written as span_emit() says. ------------------------------------------ */
                     const uint32_t code_base = sm.addr(DF_OFF_CODE), zero_ent = sm.addr(DF_OFF_CODE + DF_ZERO_SYM * 4), stage_base = sm.addr(DF_OFF_STAGE);
                     const uint32_t k4 = opaque4();
+                    uint32_t run = bitpos + hdrbits; /* bit position of the pair's first span (uniform across the CTA) */
+                    DF_PHASE_BEGIN(x_t);
 #pragma unroll
-                    for (int b = 0; b < DF_NBATCH; b++) {
-                        if ((uint32_t)b < nb) {
-                            const uint32_t sidx = (uint32_t)b * DF_THREADS + tid;
-                            const uint32_t F = fF[b], MA = fA[b], MB = ONEM ? 0u : sm.ld32(DF_OFF_REC + sidx * 8 + 4);
-                            if ((F | MA | MB) == 0) continue;
-                            const uint2 x = sm.ld64(DF_OFF_IN + sidx * DF_SPAN);
-                            uint32_t pos = base + s_bb[sidx >> 3] + sm.ld16(DF_OFF_SPN + sidx * 2); /* bit position in the staging buffer */
-                            const uint32_t ex = (F >> 8) & 3u;
-                            if (ex) {
-                                const uint32_t c0 = sm.ld32(DF_OFF_CODE + ((F >> 16) & 0xffu) * 4);
-                                stage_or(sm, pos, c0 & 0x7fffu, (c0 >> 16) & 15u);
-                                pos += (c0 >> 16) & 15u;
-                                if (ex == 2) {
-                                    const uint32_t c1 = sm.ld32(DF_OFF_CODE + (F >> 24) * 4);
-                                    stage_or(sm, pos, c1 & 0x7fffu, (c1 >> 16) & 15u);
-                                    pos += (c1 >> 16) & 15u;
-                                }
-                            }
-                            uint32_t cw[8];
-#pragma unroll
-                            for (int j = 0; j < 8; j++) {
-                                const uint32_t by = MZ_BYTE(j < 4 ? x.x : x.y, j & 3);
-                                cw[j] = sm.ld32_a(((F >> j) & 1u) ? by * k4 + code_base : zero_ent); /* code | length << 16 (a literal's entry has no extra-bits field) */
-                            }
-                            /* lengths, one per byte; a match leaves a gap of its size at its slot (slot 8 = none: the shifts clamp to 0) */
-                            const uint32_t nA = match_bits(sm, MA), nB = ONEM ? 0u : match_bits(sm, MB);
-                            const uint32_t sA = MA ? ((MA >> 28) & 7u) * 8u : 64u, sB = MB ? ((MB >> 28) & 7u) * 8u : 64u;
-                            const uint32_t L0 = __byte_perm(__byte_perm(cw[0], cw[1], 0x0062u), __byte_perm(cw[2], cw[3], 0x0062u), 0x5410u) + shl_clamp(nA, sA) + shl_clamp(nB, sB);
-                            const uint32_t L1 = __byte_perm(__byte_perm(cw[4], cw[5], 0x0062u), __byte_perm(cw[6], cw[7], 0x0062u), 0x5410u) + shl_clamp(nA, sA - 32u) + shl_clamp(nB, sB - 32u);
-                            const uint32_t P0 = L0 * 0x01010101u;                       /* inclusive sums of slots 0..3 */
-                            const uint32_t P1 = L1 * 0x01010101u + (P0 >> 24) * 0x01010101u;
-                            const uint32_t E0 = P0 << 8, E1 = __funnelshift_l(P0, P1, 8); /* exclusive: bits before slot k in byte k */
-#pragma unroll
-                            for (int jj = 0; jj < 4; jj++) {
-                                const uint32_t pp = pos + MZ_BYTE(jj < 2 ? E0 : E1, 2 * (jj & 1));
-                                /* at most the two literals are in-band, and then they are adjacent (a match start covers its neighbour) */
-                                const uint32_t c0 = cw[2 * jj], c1 = cw[2 * jj + 1];
-                                const uint32_t v = (c0 & 0xffffu) | ((c1 & 0xffffu) << (c0 >> 16));
-                                const uint32_t wa = stage_word(stage_base, pp, k4);
-                                sm.red_or32_a(wa, __funnelshift_l(0u, v, pp));
-                                sm.red_or32_a(wa + 4, __funnelshift_l(v, 0u, pp));
-                            }
-                            if (MA) put_match_bits(sm, pos + (shr_clamp(E0, sA) & 0xffu) + (shr_clamp(E1, sA - 32u) & 0xffu), MA);
-                            if (!ONEM) sm.st32(DF_OFF_REC + sidx * 8, pos + (shr_clamp(E0, sB) & 0xffu) + (shr_clamp(E1, sB - 32u) & 0xffu)); /* (only read back where MB != 0) */
-                        }
+                    for (int b = 0; b < DF_NBATCH; b += 2) {
+                        if ((uint32_t)b >= nb) break; /* (uniform) */
+                        const uint32_t s0 = (uint32_t)b * DF_THREADS + tid, s1 = s0 + DF_THREADS;
+                        /* (a short unit may end after the first batch of a pair: the second then holds nothing; its record is stale) */
+                        const uint32_t MB0 = ONEM ? 0u : sm.ld32(DF_OFF_REC + s0 * 8 + 4);
+                        const uint32_t MB1 = (ONEM || (uint32_t)b + 1 >= nb) ? 0u : sm.ld32(DF_OFF_REC + s1 * 8 + 4);
+                        const SpanBits A = span_bits<ONEM>(sm, s0, fF[b], fA[b], MB0, code_base, zero_ent, k4);
+                        const SpanBits B = span_bits<ONEM>(sm, s1, fF[b + 1], fA[b + 1], MB1, code_base, zero_ent, k4);
+                        const uint32_t sz = A.size | (B.size << 16);
+                        const uint32_t incl = warp_incl_sum(sz);
+                        if (lane == 31) s_scan[(b / 2) * DF_WARPS + warp] = incl;
+                        __syncthreads(); /* one per pair: the pair's warp totals are visible */
+                        DF_PHASE(x_t, DF_PH_X_SCAN);
+                        const uint32_t wt = lane < (unsigned)DF_WARPS ? s_scan[(b / 2) * DF_WARPS + lane] : 0u;
+                        const uint32_t wlo = wt & 0xffffu, whi = wt >> 16; /* (the sums over warps no longer fit 16 bits) */
+                        const uint32_t totA = __reduce_add_sync(MZ_FULL_MASK, wlo);
+                        const uint32_t ex = incl - sz; /* exclusive, per half (no borrow: each half of incl is at least its size) */
+                        const uint32_t posA = run + __reduce_add_sync(MZ_FULL_MASK, lane < warp ? wlo : 0u) + (ex & 0xffffu);
+                        const uint32_t posB = run + totA + __reduce_add_sync(MZ_FULL_MASK, lane < warp ? whi : 0u) + (ex >> 16);
+                        run += totA + __reduce_add_sync(MZ_FULL_MASK, whi);
+                        if (A.size) span_emit<ONEM>(sm, A, posA, s0, stage_base, k4);
+                        if (B.size) span_emit<ONEM>(sm, B, posB, s1, stage_base, k4);
+                        DF_PHASE(x_t, DF_PH_X_EMIT);
                     }
+#ifdef MZ_EMU
+                    if (run != bitpos + hdrbits + tokbits) { /* the spans' sizes must add up to what D counted from the histograms */
+                        fprintf(stderr, "deflate: block %u, unit %u: emitted %u token bits, the histograms count %u\n", (unsigned)blockIdx.x, u,
+                                run - bitpos - hdrbits, tokbits);
+                        abort();
+                    }
+#endif
                     /* ---- M3: the parked second matches, one per lane ----------------------------------------------------- */
                     if (!ONEM) {
                         uint32_t totB = 0;
@@ -1310,7 +1326,8 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                             }
                         }
                     }
-                    if (tid == DF_THREADS - 1) stage_put(s_stage, base + tokbits, eob & 0x7fffu, (eob >> 16) & 15u);
+                    DF_PHASE(x_t, DF_PH_X_M3);
+                    if (tid == DF_THREADS - 1) stage_put(s_stage, bitpos + hdrbits + tokbits, eob & 0x7fffu, (eob >> 16) & 15u);
                     bitpos += dyn_bits;
                 }
             } else {
@@ -1337,11 +1354,14 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 bitpos = (p0 + 4 + ulen) * 8;
             }
             __syncthreads();
-            DF_PHASE(ph_t, DF_PH_F_M3); /* (a stored block counts here) */
+            DF_PHASE(ph_t, DF_PH_EMIT); /* (a stored block counts here) */
             /* ---- G: flush whole 16-byte units, carry the tail ------------------------------------ */
             {
                 const uint32_t n16 = bitpos >> 7;
                 const uint32_t used_words = (bitpos + 31) >> 5;
+                /* (four copies in flight per thread; unrolled further, the copy sets the register count of the history variant,
+                 * which has no limit below 128 from its launch bounds) */
+#pragma unroll 4
                 for (uint32_t i = tid; i < n16; i += DF_THREADS) ((uint4 *)(gout + flushed))[i] = ((const uint4 *)s_stage)[i];
                 if (tid < 4) s_misc[MISC_CARRY + tid] = (n16 * 4 + tid < used_words) ? s_stage[n16 * 4 + tid] : 0u;
                 bitpos -= n16 * 128;

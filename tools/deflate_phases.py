@@ -6,7 +6,9 @@ and each phase's share, with the GPU's name, power limit and SM clock. D (the co
 barriers: stats, the two sweeps, Kraft completion (with the number of units per pass count), canonical codes, and the header. The
 parse is split at the two barriers of each batch: (a) loads, hashes and the reads of the table before the batch's inserts, (b) the
 inserts, (c) thread 0's reads after the inserts, verification, walk and record stores. M0 is split into thread 0's time in the
-capped-span index, the near-source test and the extension; the rest of M0 is the wait for the other warps.
+capped-span index, the near-source test and the extension; the rest of M0 is the wait for the other warps. The count-and-emit
+pass is split at its barrier per pair of batches: (i) code words, span sizes and the warp scan up to the barrier, (ii) thread
+0's emit of the pair, (iii) M3; the rest is the stored decision, the end-of-block code and the wait at the pass's closing barrier.
 
 The counters are thread 0's clock64() readings at the kernel's barriers, summed per CTA; cycles per unit = all CTAs' cycles over
 all units. The counting itself costs a few atomics per unit, so the kernel time printed here is not the product's.
@@ -21,7 +23,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-PHASES = ["load + hash reset", "parse batches", "M0", "cover", "T + M1", "D (codes + header)", "E + scan", "F + M3", "flush"]
+PHASES = ["load + hash reset", "parse batches", "M0", "cover", "T + M1", "D (codes + header)", "E + F + M3 (count, emit)", "flush"]
 UNITS = len(PHASES)  # column layout of g_df_phases (deflate_kernel.cuh): the phases, the unit count, D's sub-phases, the pass counts
 D_SUB = ["stats", "sweep 1", "sweep 2", "Kraft completion", "canonical codes"]  # + "header": the rest of D
 D_COL = PHASES.index("D (codes + header)")
@@ -30,8 +32,10 @@ P_SUB = ["(a) loads, hashes, old keys", "(b) inserts", "(c) verify, walk, stores
 P_COL = PHASES.index("parse batches")
 M_SUB = ["index", "near-source test", "extension"]  # + "wait": the closing barrier
 M_COL = PHASES.index("M0")
+X_SUB = ["(i) code words, sizes, scan", "(ii) emit", "(iii) M3"]  # + "rest": the stored decision, the end of block, the last barrier
+X_COL = PHASES.index("E + F + M3 (count, emit)")
 SUB0 = UNITS + 1 + len(D_SUB) + NPASS
-COLS = SUB0 + len(P_SUB) + len(M_SUB)
+COLS = SUB0 + len(P_SUB) + len(M_SUB) + len(X_SUB)
 ROWS = 1024
 
 
@@ -104,6 +108,8 @@ def main():
     psub.append(per[P_COL] - sum(psub))
     msub = [sum(r[SUB0 + len(P_SUB) + i] for r in tab) for i in range(len(M_SUB))]
     msub.append(per[M_COL] - sum(msub))
+    xsub = [sum(r[SUB0 + len(P_SUB) + len(M_SUB) + i] for r in tab) for i in range(len(X_SUB))]
+    xsub.append(per[X_COL] - sum(xsub))
     passes = [sum(r[UNITS + 1 + len(D_SUB) + i] for r in tab) // args.reps for i in range(NPASS)]  # a CTA's cycles over the launch ~ kernel time x SM clock
     res = {"gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock_after": info.get("clocks.sm"),
            "sm_clock_max": info.get("clocks.max.sm"), "level": args.level, "bytes": n, "ctas": len(tab), "units": units // args.reps,
@@ -116,6 +122,8 @@ def main():
                                for p, c in zip(P_SUB + ["rest"], psub)},
            "m0_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_m0": round(c / max(per[M_COL], 1), 4)}
                             for p, c in zip(M_SUB + ["wait"], msub)},
+           "emit_subphases": {p: {"cycles_per_unit": round(c / units, 0), "share_of_emit": round(c / max(per[X_COL], 1), 4)}
+                              for p, c in zip(X_SUB + ["rest"], xsub)},
            "kraft_passes": {("%d+" % i if i == NPASS - 1 else str(i)): n for i, n in enumerate(passes)}}
     print("%s, power limit %s, SM clock %s (max %s); effective clock during the launches %d MHz" % (
         res["gpu"], res["power_limit"], res["sm_clock_after"], res["sm_clock_max"], res["effective_sm_MHz"]))
@@ -125,7 +133,7 @@ def main():
     for p, c in zip(PHASES, per):
         print("%-30s %12.0f %6.1f%%" % (p, c / units, 100.0 * c / total))
         for col, names, sub, tag in ((D_COL, D_SUB + ["header"], dsub, "D"), (P_COL, P_SUB + ["rest"], psub, "parse"),
-                                     (M_COL, M_SUB + ["wait"], msub, "M0")):
+                                     (M_COL, M_SUB + ["wait"], msub, "M0"), (X_COL, X_SUB + ["rest"], xsub, "emit")):
             if p == PHASES[col]:
                 for q, d in zip(names, sub):
                     print("  %-28s %12.0f %6.1f%% of %s" % (q, d / units, 100.0 * d / max(per[col], 1), tag))
