@@ -323,12 +323,54 @@ typedef struct mz_cuda_zip_wr {
     uint64_t *max_csize;                   /* 1 word, 0 before entries */
     const void *digest, *salt, *keys, *mac; /* per entry: SHA-256 (sha), K8 salt / key record / HMAC (aes) */
     void *entries;                         /* mz_cuda_zip_dev_entry[n] or NULL */
+    /* what lies in front of the new entries (mz_zip_cuda_update_device; all 0 for write_device): archive bytes (added to every
+     * local-header offset, so the zip64 decision sees absolute offsets), directory bytes in front of the first new record, output
+     * bytes in front of the first new row's out_off, entries (counted in the end records); the end record's comment (device) */
+    uint64_t lh_base, cd_base, out_base;
+    uint32_t n_base, comment_len;
+    const void *comment;
 } mz_cuda_zip_wr;
 int32_t mz_cuda_zip_wr_items(const mz_cuda_zip_wr *w, uint32_t data_null, uint32_t names_null, void *stream);
 int32_t mz_cuda_zip_wr_chunks(const mz_cuda_zip_wr *w, void *stream);
 int32_t mz_cuda_zip_wr_place(const mz_cuda_zip_wr *w, uint64_t c0, uint32_t m, void *stream);
 int32_t mz_cuda_zip_wr_entries(const mz_cuda_zip_wr *w, void *stream);
 int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t cd_size, void *stream);
+
+/* ---- K13: an archive in device memory updated on the device (csrc/zipup_kernel.cuh) ---------------------------------------
+ * The device half of mz_zip_cuda_update_device (include/mz_zip_cuda.h). Slot i of n keeps entry keep[i] (keep NULL: entry i) of
+ * the source's K10 public table ent (count rows). counts: per-slot counts, their exclusive scan pre[0..n] (pre[i].ext is slot i's
+ * new local-header offset), then info: [0] the first slot whose offset needs the zip64 field (>= n: none), [1] the first keep index
+ * >= count, [2] the first slot whose bytes move or whose extent holds more than its local header, stored bytes and data descriptor, [3] the first slot whose record would pass 65535 bytes of extra field, [4] / [5]
+ * the source's end record and its comment length; [0..3] are ~0 before the call when nothing applies. `part`: scan scratch of
+ * (n / MZ_CUDA_ZIP_WR_TILE + 1) counts. copy: every slot's extent (local header, stored bytes, descriptor) from src to archive +
+ * pre[i].ext, stores below cap only; a slot whose destination is its source is skipped. records: slot i's directory record at
+ * cd_off + pre[i].cd + 28 x (slots in front of i from info[0] on), its mz_cuda_zip_dev_entry row to entries[i] (if not NULL). The
+ * records are read from dir + (record offset - dir_off): the source itself (dir = src + dir_off) or a saved copy of its tail. */
+typedef struct mz_cuda_zip_up_count { /* per slot; pre[i] = the sum over the slots in front of i */
+    uint64_t ext;       /* the entry's extent */
+    uint64_t cd;        /* its directory record without zip64 fields */
+    uint64_t out16;     /* plain bytes rounded up to 16 */
+    uint64_t bytes;     /* plain bytes */
+    uint64_t stored;    /* stored bytes */
+} mz_cuda_zip_up_count;
+#define MZ_CUDA_ZIP_UP_INFO 6
+typedef struct mz_cuda_zip_up {
+    const void *src;                       /* the source archive */
+    const void *ent;                       /* its mz_cuda_zip_dev_entry table (K10) */
+    uint32_t count, n;
+    const uint32_t *keep;
+    const void *dir;
+    uint64_t dir_off, src_len;
+    mz_cuda_zip_up_count *cnt, *pre;       /* n, n + 1 */
+    void *part;
+    uint64_t *info;                        /* MZ_CUDA_ZIP_UP_INFO words */
+    void *archive;
+    uint64_t cap, cd_off;
+    void *entries;
+} mz_cuda_zip_up;
+int32_t mz_cuda_zip_up_counts(const mz_cuda_zip_up *u, void *stream);
+int32_t mz_cuda_zip_up_copy(const mz_cuda_zip_up *u, void *stream);
+int32_t mz_cuda_zip_up_records(const mz_cuda_zip_up *u, void *stream);
 
 /* ---- K6: one long foreign stream, segment-speculative (csrc/inflate_spec_kernel.cuh) ------------------------
  * One ROUND decodes as much of the compressed window d_in[0..in_avail) as can be proven, starting at the block

@@ -251,6 +251,46 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
                                  const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
                                  mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream);
 
+/* ---- an archive in device memory updated on the device ----------------------------------------------------------------
+ * Keeps, drops and appends entries of an archive in device memory without recompressing the kept ones: what the reference's append
+ * mode (mz_zip_open with MZ_OPEN_MODE_APPEND, mz_zip.c:1445) and `minizip -e` (raw copies through mz_zip_writer_copy_from_reader,
+ * mz_zip_rw.c:1731) do on the host, on the device (K10 parses the source, K13 moves the kept entries and rewrites their records,
+ * K11 writes the new entries, csrc/zipup_kernel.cuh). Synchronous on `stream`.
+ *   - output: (1) the kept entries of d_src[0, src_len), in keep order, each its raw extent (local header, stored bytes, any data
+ *     descriptor: unchanged); (2) the count new entries, exactly as write_device lays them out; (3) the directory: the kept records,
+ *     then the new ones; (4) a zip64 end record and locator when the directory starts at 0xffffffff or later or there are 65535
+ *     entries or more (write_device's rule); (5) the end record with the source's archive comment. Data in front of the source's
+ *     first entry (a self-extracting stub) is not carried over.
+ *   - d_keep NULL (nkeep 0): every accepted entry, in directory order (append). Otherwise nkeep indices into the source's accepted
+ *     entries (the rows extract_device and the reader list), any order, repeats allowed.
+ *   - errors, in this order, and nothing is written when one of them is returned: (1) write_device's argument errors, then d_src NULL
+ *     with src_len > 0, d_keep NULL with nkeep > 0, and overlapping buffers other than in place (below): MZ_PARAM_ERROR; (2) an error
+ *     of the source as a whole, exactly as extract_device returns it (the parse runs as if a password had been given: nothing is
+ *     decrypted); (3) a refused record (PKWARE encryption, another method, an entry above 1 GiB...): its code, not a shorter list;
+ *     (4) a keep index >= the accepted count: MZ_PARAM_ERROR; in place, entries that do not tile [0, directory): MZ_PARAM_ERROR;
+ *     a kept record that needs the zip64 field but whose extra field would pass 65535 bytes: MZ_SUPPORT_ERROR; (5) item errors, as
+ *     write_device reports them.
+ *   - kept WinZip AES entries are copied still encrypted: no password is needed for them. password and aes_strength apply to the
+ *     new entries with MZ_ZIP_CUDA_AES only; flags as write_device (MZ_ZIP_CUDA_HASH_SHA256 allowed, MZ_ZIP_CUDA_ALL_DEVICES:
+ *     MZ_PARAM_ERROR).
+ *   - kept records: fixed fields, name, file comment and every extra field but zip64 (0x0001) unchanged and in order; the local-header
+ *     offset becomes the entry's new one; the source's zip64 fields are dropped; when the new offset is 0xffffffff or more, sizes and
+ *     offset are saturated and a 28-byte zip64 field follows the name, as write_device writes it. Version needed becomes at least
+ *     45 with a zip64 field, and goes back to 20 for a non-AES record at 45 that loses its zip64 field. The disk number is written
+ *     as 0. So a record write_device wrote comes out as write_device would write it at its new offset.
+ *   - d_archive == NULL: sizing call, *archive_len = an upper bound. cap too small: MZ_BUF_ERROR with *archive_len = the exact length
+ *     (bytes below cap may have been written). No byte at or beyond cap is ever written. d_entries (optional, device): the
+ *     nkeep + count rows extract_device lists for the output.
+ *   - in place: d_archive == d_src only with d_keep NULL and entries that tile [0, directory) exactly (no prepended data, no gaps).
+ *     The kept bytes are not moved and writing starts at the old directory, as the reference's append does. The bytes from the
+ *     source's directory to src_len are saved first; on any later error (MZ_BUF_ERROR, MZ_INTERNAL_ERROR, ...) they are put back, so
+ *     a failed call leaves the source a valid archive.
+ *   - stats: as write_device, entries / bytes_* over the whole output; pack_ms = the parse and planning. */
+int32_t mz_zip_cuda_update_device(const void *d_src, uint64_t src_len, const uint32_t *d_keep, uint32_t nkeep, const void *d_data, const void *d_names,
+                                  const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags, const char *password,
+                                  uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len, mz_cuda_zip_dev_entry *d_entries,
+                                  mz_cuda_zip_stats *stats, void *stream);
+
 /* sizeof the mz_zip_file mirror this library was built with: the host asserts it equals sizeof(mz_zip_file) */
 uint32_t mz_zip_cuda_abi_file_info_size(void);
 

@@ -60,6 +60,7 @@ EXPORTS = [
     "mz_zip_cuda_add_buffers", "mz_zip_cuda_add_buffers_ex", "mz_zip_cuda_write_archive", "mz_zip_cuda_trim", "mz_zip_cuda_write_archive_aes", "mz_zip_cuda_extract_all",
     "mz_zip_cuda_extract_all_aes", "mz_zip_cuda_extract_archive", "mz_zip_cuda_extract_device", "mz_zip_cuda_write_device", "mz_zip_cuda_abi_file_info_size",
     "mz_zip_cuda_reader_open", "mz_zip_cuda_reader_entries", "mz_zip_cuda_reader_locate", "mz_zip_cuda_reader_decode", "mz_zip_cuda_reader_close",
+    "mz_zip_cuda_update_device",
     # include/mz_cuda_batch.h, K9 and K10
     "mz_cuda_zip_locate", "mz_cuda_zip_copy_stored", "mz_cuda_zip_verify", "mz_cuda_zip_parse_directory", "mz_cuda_zip_statuses",
     # include/mz_cuda_batch.h, K11
@@ -67,6 +68,8 @@ EXPORTS = [
     # include/mz_cuda_batch.h, K12
     "mz_cuda_zip_name_index", "mz_cuda_zip_name_lookup", "mz_cuda_zip_sel_counts", "mz_cuda_zip_sel_fill", "mz_cuda_zip_sel_gather",
     "mz_cuda_zip_sel_status",
+    # include/mz_cuda_batch.h, K13
+    "mz_cuda_zip_up_counts", "mz_cuda_zip_up_copy", "mz_cuda_zip_up_records",
 ]
 
 # mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
@@ -195,6 +198,8 @@ def configure(L):
     sig("mz_zip_cuda_trim", None, [])
     sig("mz_zip_cuda_extract_device", i32, [vp, u64, C.c_char_p, vp, u32, C.POINTER(u32), vp, u64, C.POINTER(u64), vp, vp])
     sig("mz_zip_cuda_write_device", i32, [vp, vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp, u64, C.POINTER(u64), vp, vp, vp])
+    sig("mz_zip_cuda_update_device", i32, [vp, u64, vp, u32, vp, vp, vp, u32, C.c_int16, u32, C.c_char_p, C.c_uint8, vp, u64, C.POINTER(u64), vp, vp,
+                                           vp])
     sig("mz_cuda_zip_parse_directory", i32, [vp, u64, vp, vp])
     sig("mz_cuda_zip_statuses", i32, [vp, u32, vp, vp, vp])
     sig("mz_zip_cuda_reader_open", i32, [vp, u64, C.c_char_p, C.POINTER(vp), C.POINTER(u32), C.POINTER(i32), vp, vp])
@@ -416,12 +421,27 @@ def write_device(files, level=6, sha256=False, password=None, aes_strength=3, mt
     tensor)], all on the current device; the tensors may be separate allocations. The archive is what write_archive writes for the same
     bytes (with a password: WinZip AES of aes_strength). mtime: unix time of every entry (None = now). Returns a CUDA uint8 tensor of
     exactly the archive's length. Raises on any error, as check() does."""
-    import time
     import torch
     lib = load()
     check(lib.mz_cuda_init(), "mz_cuda_init")
     dev = torch.device("cuda", torch.cuda.current_device())
     flags = (MZ_ZIP_CUDA_HASH_SHA256 if sha256 else 0) | (MZ_ZIP_CUDA_AES if password is not None else 0)
+    base, d_names, d_items = _dev_items(files, dev, mtime)
+    pw = password.encode() if password is not None else None
+    s = _stream_ptr()
+    n = C.c_uint64(0)
+    args = (base or None, d_names.data_ptr(), d_items.data_ptr(), len(files), level, flags, pw, aes_strength)
+    check(lib.mz_zip_cuda_write_device(*args, None, 0, C.byref(n), None, None, s), "write_device")  # sizing: an upper bound
+    out = torch.empty(max(1, n.value), dtype=torch.uint8, device=dev)
+    check(lib.mz_zip_cuda_write_device(*args, out.data_ptr(), n.value, C.byref(n), None, None, s), "write_device")
+    return out[:n.value].clone()  # the bound-sized buffer is released: the archive's own storage is exactly its length
+
+
+def _dev_items(files, dev, mtime):
+    """-> (base, d_names, d_items): the mz_cuda_zip_dev_item table of files = [(name, CUDA uint8 tensor)] on dev, data offsets from
+    base (the lowest data pointer, 0 without data); the tensors in `files` must stay alive while the table is used"""
+    import time
+    import torch
     date = dos_date(int(time.time() if mtime is None else mtime))
     tensors = []
     for name, t in files:
@@ -438,14 +458,50 @@ def write_device(files, level=6, sha256=False, password=None, aes_strength=3, mt
         items[i] = ZipDevItem(t.data_ptr() - base if t.numel() else 0, t.numel(), pos, len(nm), date, 0, 0)
         pos += len(nm)
     d_items = torch.frombuffer(bytearray(bytes(items)), dtype=torch.uint8).to(dev)
+    return base, d_names, d_items
+
+
+def update_device(archive, keep=None, files=(), level=6, sha256=False, password=None, aes_strength=3, mtime=None):
+    """Update a zip archive held in a CUDA uint8 tensor without recompressing the entries it keeps (mz_zip_cuda_update_device): the
+    kept entries are copied as raw bytes and their directory records rewritten, then `files` (as write_device takes them) are appended.
+    keep: None keeps every entry (append); otherwise entry indices as ZipDeviceReader.entries and .locate give them (a list, or a CPU
+    or CUDA integer tensor; any order, repeats allowed; empty keeps none), or a boolean mask over the entries (the entries where it is
+    True, in order), e.g. a locate followed by a mask to drop files by name. Kept WinZip AES entries
+    stay encrypted under their own password; `password` applies to the new entries. The archive's comment is kept. Returns a new CUDA
+    uint8 tensor of exactly the archive's length; `archive` is not changed. Raises on any error, as check() does."""
+    import torch
+    lib = load()
+    check(lib.mz_cuda_init(), "mz_cuda_init")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    assert archive.is_cuda and archive.dtype == torch.uint8 and archive.device == dev, "archive: a CUDA uint8 tensor on the current device"
+    src = archive.contiguous()
+    d_keep, nkeep = None, 0
+    if keep is not None:
+        k = torch.as_tensor(keep)
+        if k.numel() == 0:  # [] comes as float32: an empty list of indices
+            k = torch.empty(0, dtype=torch.int64)
+        if k.dtype == torch.bool:  # a mask over the entries: keep the entries it selects
+            k = k.reshape(-1).nonzero().reshape(-1)
+        if k.is_floating_point() or k.is_complex():
+            raise TypeError("update_device: keep holds entry indices or a boolean mask")
+        k = k.to(torch.int64).reshape(-1)
+        if k.numel() and bool((k < 0).any()):
+            raise ValueError("update_device: negative entry index")
+        # never NULL: the C call reads a NULL d_keep as "keep every entry", an empty list keeps none
+        d_keep = torch.zeros(max(1, k.numel()), dtype=torch.int32, device=dev)
+        d_keep[:k.numel()] = k.to(torch.int32).to(dev)
+        nkeep = k.numel()
+    flags = (MZ_ZIP_CUDA_HASH_SHA256 if sha256 else 0) | (MZ_ZIP_CUDA_AES if password is not None else 0)
+    base, d_names, d_items = _dev_items(files, dev, mtime)
     pw = password.encode() if password is not None else None
     s = _stream_ptr()
     n = C.c_uint64(0)
-    args = (base or None, d_names.data_ptr(), d_items.data_ptr(), len(files), level, flags, pw, aes_strength)
-    check(lib.mz_zip_cuda_write_device(*args, None, 0, C.byref(n), None, None, s), "write_device")  # sizing: an upper bound
+    args = (src.data_ptr() if src.numel() else None, src.numel(), d_keep.data_ptr() if d_keep is not None else None, nkeep,
+            base or None, d_names.data_ptr(), d_items.data_ptr(), len(files), level, flags, pw, aes_strength)
+    check(lib.mz_zip_cuda_update_device(*args, None, 0, C.byref(n), None, None, s), "update_device")  # sizing: an upper bound
     out = torch.empty(max(1, n.value), dtype=torch.uint8, device=dev)
-    check(lib.mz_zip_cuda_write_device(*args, out.data_ptr(), n.value, C.byref(n), None, None, s), "write_device")
-    return out[:n.value].clone()  # the bound-sized buffer is released: the archive's own storage is exactly its length
+    check(lib.mz_zip_cuda_update_device(*args, out.data_ptr(), n.value, C.byref(n), None, None, s), "update_device")
+    return out[:n.value].clone()
 
 
 def inflate_device(comp, out_cap):

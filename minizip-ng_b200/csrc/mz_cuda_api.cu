@@ -22,6 +22,7 @@
 #include "zipcd_kernel.cuh"
 #include "zipwr_kernel.cuh"
 #include "zipsel_kernel.cuh"
+#include "zipup_kernel.cuh"
 #include "../../include/mz_zip_cuda.h"
 
 #define MZ_OK 0
@@ -43,11 +44,15 @@ static_assert(sizeof(mz_cuda_zip_dev_entry) == sizeof(ZipDevEnt) && sizeof(mz_cu
               "device zip entry layout");
 static_assert(sizeof(mz_cuda_zip_dev_item) == sizeof(ZwItem) && sizeof(ZwItem) == 40 && sizeof(mz_cuda_zip_wr_count) == sizeof(ZwCount) &&
                   sizeof(mz_cuda_zip_wr) == sizeof(ZwCall) && offsetof(mz_cuda_zip_wr, entries) == offsetof(ZwCall, entries) &&
+                  offsetof(mz_cuda_zip_wr, comment) == offsetof(ZwCall, comment) &&
                   MZ_CUDA_ZIP_WR_TILE == ZC_TILE,
               "device zip writer layout");
 static_assert(sizeof(mz_cuda_zip_sel_count) == sizeof(ZsCount) && sizeof(ZsCount) == 56 && sizeof(mz_cuda_zip_sel) == sizeof(ZsCall) &&
                   offsetof(mz_cuda_zip_sel, scratch) == offsetof(ZsCall, scratch),
               "device zip selection layout");
+static_assert(sizeof(mz_cuda_zip_up_count) == sizeof(ZuCount) && sizeof(mz_cuda_zip_up) == sizeof(ZuCall) &&
+                  offsetof(mz_cuda_zip_up, entries) == offsetof(ZuCall, entries) && MZ_CUDA_ZIP_UP_INFO == ZU_NINFO,
+              "device zip update layout");
 
 namespace {
 
@@ -807,7 +812,59 @@ int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t c
     const cudaStream_t s = (cudaStream_t)stream;
     const uint32_t per = ZW_THREADS / 32;
     if (W.n) MZ_LAUNCH(zw_emit_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, cd_off);
-    MZ_LAUNCH(zw_end_kernel, dim3(1), dim3(1), 0, s, W, cd_off, cd_size);
+    MZ_LAUNCH(zw_end_kernel, dim3(1), dim3(ZW_THREADS), 0, s, W, cd_off, cd_size);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+/* ---- K13: an archive in device memory updated on the device ------------------------------------------------------ */
+extern "C++" {
+namespace {
+ZuCall zu_call(const mz_cuda_zip_up *u) {
+    ZuCall U;
+    memcpy(&U, u, sizeof(U));
+    return U;
+}
+} // namespace
+} // extern "C++"
+
+int32_t mz_cuda_zip_up_counts(const mz_cuda_zip_up *u, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!u || !u->cnt || !u->pre || !u->part || !u->info || !u->src || (u->n && (!u->dir || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
+    const ZuCall U = zu_call(u);
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t g = (U.n + ZU_THREADS - 1) / ZU_THREADS;
+    if (U.n) MZ_LAUNCH(zu_counts_kernel, dim3(g), dim3(ZU_THREADS), 0, s, U);
+    CK(cudaGetLastError());
+    if ((err = zw_scan<ZuCount>(U.cnt, U.n, U.pre, (ZuCount *)U.part, s))) return err;
+    if (U.n) MZ_LAUNCH(zu_layout_kernel, dim3(g), dim3(ZU_THREADS), 0, s, U);
+    MZ_LAUNCH(zu_comment_kernel, dim3(1), dim3(ZU_THREADS), 0, s, U);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_up_copy(const mz_cuda_zip_up *u, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!u || !u->pre || !u->archive || (u->n && (!u->src || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
+    if (u->n == 0) return MZ_OK;
+    const uint32_t per = ZU_THREADS / 32, g = (u->n + per - 1) / per, cap = (uint32_t)c->sm_count * 8u;
+    MZ_LAUNCH(zu_copy_kernel, dim3(g < cap ? g : cap), dim3(ZU_THREADS), 0, (cudaStream_t)stream, zu_call(u));
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_zip_up_records(const mz_cuda_zip_up *u, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!u || !u->pre || !u->info || !u->archive || (u->n && (!u->dir || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
+    if (u->n == 0) return MZ_OK;
+    const uint32_t per = ZU_THREADS / 32;
+    MZ_LAUNCH(zu_records_kernel, dim3((u->n + per - 1) / per), dim3(ZU_THREADS), 0, (cudaStream_t)stream, zu_call(u));
     CK(cudaGetLastError());
     return MZ_OK;
 }

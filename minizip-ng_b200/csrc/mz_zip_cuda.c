@@ -2393,32 +2393,50 @@ void mz_zip_cuda_reader_close(mz_zip_cuda_dev_reader *r) {
     free(r);
 }
 
-int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags,
-                                 const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
-                                 mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream) {
-    mz_cuda_zip_stats st;
-    memset(&st, 0, sizeof(st));
-    if (stats)
-        *stats = st;
-    /* the host writer's order: options, pointers, level, password and strength, the GPU */
+/* the argument checks of write_device, in the host writer's order: options, pointers, level, password and strength, the GPU; *level and
+ * *aes_strength get their defaults */
+static int32_t zw_args(const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t *level, uint32_t flags, const char *password,
+                       uint8_t *aes_strength, uint64_t *archive_len) {
     if (flags & ~(MZ_ZIP_CUDA_HASH_SHA256 | MZ_ZIP_CUDA_AES))
         return MZ_PARAM_ERROR; /* MZ_ZIP_CUDA_ALL_DEVICES among them: the entries live on one device */
     if (!archive_len || (!d_items && count))
         return MZ_PARAM_ERROR;
     *archive_len = 0;
-    if (level == MZ_COMPRESS_LEVEL_DEFAULT)
-        level = 6;
-    if (level < 0 || level > 9)
+    if (*level == MZ_COMPRESS_LEVEL_DEFAULT)
+        *level = 6;
+    if (*level < 0 || *level > 9)
         return MZ_PARAM_ERROR;
-    const int aes = (flags & MZ_ZIP_CUDA_AES) != 0;
-    if (aes_strength == 0)
-        aes_strength = 3;
-    if (aes && (!password || strlen(password) > 128 || aes_strength > 3))
+    if (*aes_strength == 0)
+        *aes_strength = 3;
+    if ((flags & MZ_ZIP_CUDA_AES) && (!password || strlen(password) > 128 || *aes_strength > 3))
         return MZ_PARAM_ERROR;
     if (mz_cuda_init() != MZ_OK) {
         fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
         return MZ_SUPPORT_ERROR;
     }
+    return MZ_OK;
+}
+
+/* what lies in front of the new entries: the kept entries of mz_zip_cuda_update_device; all zero for write_device */
+typedef struct zw_front {
+    uint64_t lh, cd, out;            /* archive bytes, directory bytes (zip64 fields included), 16-byte output slots */
+    uint32_t n, comment_len;         /* entries; the end record's comment */
+    const void *comment;             /* device; read when the end records are written */
+    uint64_t bytes_in, bytes_out;    /* plain and stored bytes of those entries (stats) */
+    /* called once the items passed and the call writes (before anything is written), and once the exact length fits cap (cd_off:
+     * where the directory starts) */
+    int32_t (*before)(void *ctx, void *stream);
+    int32_t (*records)(void *ctx, uint64_t cd_off, void *stream);
+    void *ctx;
+} zw_front;
+
+/* the body of write_device, behind f (arguments checked by zw_args; st zeroed) */
+static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level,
+                        uint32_t flags, const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
+                        mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats_out, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    const int aes = (flags & MZ_ZIP_CUDA_AES) != 0;
     const double t0 = now_ms();
     mz_cuda_zip_wr w;
     memset(&w, 0, sizeof(w));
@@ -2431,7 +2449,11 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
     w.dos_now = za_dos_date(0);
     w.archive = d_archive;
     w.cap = d_archive ? cap : 0;
-    w.entries = d_entries;
+    w.entries = d_entries ? d_entries + f->n : NULL;
+    w.lh_base = f->lh;
+    w.cd_base = f->cd;
+    w.out_base = f->out;
+    w.n_base = f->n;
     const size_t m = (size_t)count + 1, tiles = (size_t)count / MZ_CUDA_ZIP_WR_TILE + 1;
     /* 1. validation and per-item counts: the first invalid item and the totals come back */
     const size_t sz1[4] = {16, m * sizeof(mz_cuda_zip_wr_count), m * sizeof(mz_cuda_zip_wr_count), tiles * sizeof(mz_cuda_zip_wr_count)};
@@ -2439,8 +2461,10 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
     double ts = now_ms();
     uint8_t *work1 = zw_carve(sz1, p1, 4), *work2 = NULL;
     st.setup_ms += now_ms() - ts;
-    if (!work1)
+    if (!work1) {
+        *stats_out = st;
         return MZ_MEM_ERROR;
+    }
     int32_t err = mz_cuda_memset(w.bad, 0xff, 8, stream);
     if (!err) err = mz_cuda_zip_wr_items(&w, d_data == NULL, d_names == NULL, stream);
     uint64_t bad = ~0ull;
@@ -2452,17 +2476,19 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
     if (!err && bad != ~0ull)
         err = (bad & 1) ? MZ_SUPPORT_ERROR : MZ_PARAM_ERROR;
     if (!err && !d_archive) { /* sizing: the slot bound of every chunk, exact headers; the zip64 fields only when an offset can need them */
-        const int big = tot.overhead + tot.bound >= 0xffffffffull;
-        *archive_len = tot.overhead + tot.bound + tot.cd + (big ? 28ull * count : 0) + 22 + (big || count >= 0xffffu ? 76 : 0);
+        const int big = f->lh + tot.overhead + tot.bound >= 0xffffffffull;
+        *archive_len = f->lh + tot.overhead + tot.bound + f->cd + tot.cd + (big ? 28ull * count : 0) + 22 + f->comment_len +
+                       (big || (uint64_t)f->n + count >= 0xffffu ? 76 : 0);
     }
     st.pack_ms = now_ms() - t0 - st.setup_ms; /* the scratch allocation is setup_ms */
     if (err || !d_archive) {
         mz_cuda_stream_sync(stream);
         mz_cuda_free(work1);
-        if (stats)
-            *stats = st;
+        *stats_out = st;
         return err;
     }
+    if (f->before)
+        err = f->before(f->ctx, stream);
     /* 2. scratch: the chunk table, a round of slots, per-entry arrays */
     size_t round_bytes = (size_t)1024 << 20;
     {
@@ -2490,9 +2516,10 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
                      (void **)&w.e_off, (void **)&w.e_len, (void **)&w.e_crc, (void **)&w.max_csize, &part2, (void **)&slots, &digest, &salt, &keys, &mac,
                      (void **)&pw, &spare};
     ts = now_ms();
-    work2 = zw_carve(sz2, p2, 26);
+    if (!err)
+        work2 = zw_carve(sz2, p2, 26);
     st.setup_ms += now_ms() - ts;
-    if (!work2)
+    if (!err && !work2)
         err = MZ_MEM_ERROR;
     w.part = part2;
     w.digest = digest;
@@ -2522,8 +2549,8 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
     if (!err) err = mz_cuda_memcpy_d2h(&max_csize, w.max_csize, 8, stream);
     if (!err) err = mz_cuda_memcpy_d2h(&bad, w.bad, 8, stream);
     if (!err) err = mz_cuda_stream_sync(stream);
-    const uint64_t cd_off = tot.overhead + streams;
-    const uint64_t len = cd_off + cd_size + 22 + (cd_off >= 0xffffffffull || count >= 0xffffu ? 76 : 0);
+    const uint64_t cd_off = f->lh + tot.overhead + streams, ntot = (uint64_t)f->n + count;
+    const uint64_t len = cd_off + f->cd + cd_size + 22 + f->comment_len + (cd_off >= 0xffffffffull || ntot >= 0xffffu ? 76 : 0);
     if (!err && bad != ~0ull)
         err = MZ_INTERNAL_ERROR; /* an entry's stored size does not fit its local header: what za_prepare returns for it */
     if (!err) {
@@ -2552,17 +2579,189 @@ int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const 
         if (!err) err = mz_cuda_wzaes_ctr(d_archive, w.e_coff, w.e_csize, count, max_csize, keys, aes_strength, stream);
         if (!err) err = mz_cuda_wzaes_hmac(d_archive, w.e_coff, w.e_csize, count, keys, aes_strength, mac, stream);
     }
-    if (!err) err = mz_cuda_zip_wr_emit(&w, cd_off, cd_size, stream);
+    if (!err && f->records) err = f->records(f->ctx, cd_off, stream);
+    w.comment = f->comment;
+    w.comment_len = f->comment_len;
+    if (!err) err = mz_cuda_zip_wr_emit(&w, cd_off, f->cd + cd_size, stream);
     if (!err) err = mz_cuda_stream_sync(stream);
     st.gpu_ms = now_ms() - t1;
     if (!err || err == MZ_BUF_ERROR) {
-        st.entries = count;
-        st.bytes_in = tot.bytes;
-        st.bytes_out = streams + (aes ? (uint64_t)count * (4u * aes_strength + 4u + 2u + 10u) : 0);
+        st.entries = f->n + count;
+        st.bytes_in = f->bytes_in + tot.bytes;
+        st.bytes_out = f->bytes_out + streams + (aes ? (uint64_t)count * (4u * aes_strength + 4u + 2u + 10u) : 0);
     }
     mz_cuda_stream_sync(stream);
     mz_cuda_free(work2);
     mz_cuda_free(work1);
+    *stats_out = st;
+    return err;
+}
+
+int32_t mz_zip_cuda_write_device(const void *d_data, const void *d_names, const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags,
+                                 const char *password, uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len,
+                                 mz_cuda_zip_dev_entry *d_entries, mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    int32_t err = zw_args(d_items, count, &level, flags, password, &aes_strength, archive_len);
+    if (err)
+        return err;
+    zw_front f;
+    memset(&f, 0, sizeof(f));
+    err = zw_write(&f, d_data, d_names, d_items, count, level, flags, password, aes_strength, d_archive, cap, archive_len, d_entries, &st, stream);
+    if (stats)
+        *stats = st;
+    return err;
+}
+
+/* ---- an archive in device memory updated on the device (mz_zip_cuda_update_device) ---------------------------------------- */
+typedef struct zu_job {
+    mz_cuda_zip_up u;
+    uint64_t cd_off, src_len;   /* the source's directory; its length */
+    int in_place;
+    uint8_t *saved;             /* in place: the source's bytes from its directory on */
+    uint64_t eocd;              /* the source's end record */
+    zw_front *f;
+} zu_job;
+
+/* before anything is written: in place, save the source's directory and tail (the records and the comment are read from there);
+ * then move the kept entries */
+static int32_t zu_before(void *ctx, void *stream) {
+    zu_job *j = (zu_job *)ctx;
+    int32_t err = MZ_OK;
+    if (j->in_place) {
+        const uint64_t tail = j->src_len - j->cd_off;
+        if (!(j->saved = (uint8_t *)mz_cuda_malloc(tail ? tail : 1)))
+            return MZ_MEM_ERROR;
+        if (tail) err = mz_cuda_memcpy_d2d(j->saved, (const uint8_t *)j->u.src + j->cd_off, tail, stream);
+        j->u.dir = j->saved;
+        j->f->comment = j->saved + (j->eocd + 22 - j->cd_off);
+    }
+    if (!err) err = mz_cuda_zip_up_copy(&j->u, stream);
+    return err;
+}
+
+static int32_t zu_records(void *ctx, uint64_t cd_off, void *stream) {
+    zu_job *j = (zu_job *)ctx;
+    j->u.cd_off = cd_off;
+    return mz_cuda_zip_up_records(&j->u, stream);
+}
+
+int32_t mz_zip_cuda_update_device(const void *d_src, uint64_t src_len, const uint32_t *d_keep, uint32_t nkeep, const void *d_data, const void *d_names,
+                                  const mz_cuda_zip_dev_item *d_items, uint32_t count, int16_t level, uint32_t flags, const char *password,
+                                  uint8_t aes_strength, void *d_archive, uint64_t cap, uint64_t *archive_len, mz_cuda_zip_dev_entry *d_entries,
+                                  mz_cuda_zip_stats *stats, void *stream) {
+    mz_cuda_zip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    /* 1. arguments: write_device's, then the source and the two buffers */
+    int32_t err = zw_args(d_items, count, &level, flags, password, &aes_strength, archive_len);
+    if (err)
+        return err;
+    if ((!d_src && src_len) || (!d_keep && nkeep))
+        return MZ_PARAM_ERROR;
+    const uintptr_t s0 = (uintptr_t)d_src, a0 = (uintptr_t)d_archive;
+    const int in_place = d_archive && a0 == s0;
+    if (in_place && d_keep)
+        return MZ_PARAM_ERROR;
+    if (d_archive && !in_place && cap && a0 < s0 + src_len && s0 < a0 + cap)
+        return MZ_PARAM_ERROR; /* partly overlapping buffers */
+    const double t0 = now_ms();
+    /* 2. the source's directory (K10): nothing is decrypted, so it is parsed as if a password had been given */
+    mz_cuda_zip_dir dir;
+    memset(&dir, 0, sizeof(dir));
+    dir.have_password = 1;
+    dir.max_entries = 0xffffffffu;
+    dir.alloc_entries = 1;
+    err = mz_cuda_zip_parse_directory(d_src, src_len, &dir, stream);
+    if (err == MZ_OK && dir.err)
+        err = dir.err;
+    if (err == MZ_OK && dir.refuse)
+        err = dir.refuse; /* a refused record: the entries behind it are not dropped silently */
+    const uint32_t n = d_keep ? nkeep : dir.count;
+    zu_job j;
+    memset(&j, 0, sizeof(j));
+    zw_front f;
+    memset(&f, 0, sizeof(f));
+    j.f = &f;
+    j.cd_off = dir.cd_off;
+    j.src_len = src_len;
+    j.in_place = in_place;
+    mz_cuda_zip_up *u = &j.u;
+    u->src = d_src;
+    u->ent = dir.entries;
+    u->count = dir.count;
+    u->n = n;
+    u->keep = d_keep;
+    u->dir = (const uint8_t *)d_src + dir.cd_off;
+    u->dir_off = dir.cd_off;
+    u->src_len = src_len;
+    u->archive = d_archive;
+    u->cap = d_archive ? cap : 0;
+    u->entries = d_entries;
+    /* 3. kept counts, their scan and the layout facts; one readback */
+    uint8_t *work = NULL;
+    if (!err) {
+        const size_t m = (size_t)n + 1;
+        const size_t sz[4] = {m * sizeof(mz_cuda_zip_up_count), m * sizeof(mz_cuda_zip_up_count),
+                              ((size_t)n / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_up_count), 8 * MZ_CUDA_ZIP_UP_INFO};
+        void **p[4] = {(void **)&u->cnt, (void **)&u->pre, &u->part, (void **)&u->info};
+        const double ts = now_ms();
+        work = zw_carve(sz, p, 4);
+        st.setup_ms += now_ms() - ts;
+        if (!work)
+            err = MZ_MEM_ERROR;
+    }
+    mz_cuda_zip_up_count tot;
+    memset(&tot, 0, sizeof(tot));
+    uint64_t info[MZ_CUDA_ZIP_UP_INFO];
+    memset(info, 0, sizeof(info));
+    if (!err) err = mz_cuda_memset(u->info, 0xff, 8 * MZ_CUDA_ZIP_UP_INFO, stream);
+    if (!err) err = mz_cuda_memset(u->info + 4, 0, 16, stream);
+    if (!err) err = mz_cuda_zip_up_counts(u, stream);
+    if (!err) err = mz_cuda_memcpy_d2h(&tot, u->pre + n, sizeof(tot), stream);
+    if (!err) err = mz_cuda_memcpy_d2h(info, u->info, sizeof(info), stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    /* 4. a keep index out of range; in place, kept bytes that would move or a directory that does not start where they end */
+    if (!err && info[1] != ~0ull)
+        err = MZ_PARAM_ERROR;
+    if (!err && in_place && (info[2] != ~0ull || tot.ext != dir.cd_off))
+        err = MZ_PARAM_ERROR;
+    if (!err && info[3] != ~0ull)
+        err = MZ_SUPPORT_ERROR; /* a kept record's extra field cannot take the zip64 field it needs */
+    const uint64_t first64 = info[0] < n ? info[0] : n;
+    f.lh = tot.ext;
+    f.cd = tot.cd + 28ull * (n - first64);
+    f.out = tot.out16;
+    f.n = n;
+    f.comment_len = (uint32_t)info[5];
+    f.comment = (const uint8_t *)d_src + info[4] + 22;
+    f.bytes_in = tot.bytes;
+    f.bytes_out = tot.stored;
+    f.before = zu_before;
+    f.records = zu_records;
+    f.ctx = &j;
+    const double parse_ms = now_ms() - t0 - st.setup_ms, setup_ms = st.setup_ms;
+    j.eocd = info[4];
+    if ((uint64_t)n + count > 0xffffffffull && !err)
+        err = MZ_PARAM_ERROR;
+    /* 5. - 9. the items, [sizing], the save and the copy, the new entries, the records, the end records: write_device's body */
+    if (!err)
+        err = zw_write(&f, d_data, d_names, d_items, count, level, flags, password, aes_strength, d_archive, cap, archive_len, d_entries, &st, stream);
+    st.pack_ms += parse_ms;
+    st.setup_ms += setup_ms;
+    if (err && j.saved) { /* put the source's directory and tail back: the source stays a valid archive */
+        const uint64_t end = src_len < cap ? src_len : cap;
+        if (end > j.cd_off) mz_cuda_memcpy_d2d((uint8_t *)d_src + j.cd_off, j.saved, end - j.cd_off, stream);
+    }
+    mz_cuda_stream_sync(stream);
+    mz_cuda_free(j.saved);
+    mz_cuda_free(work);
+    mz_cuda_free(dir.entries);
+    mz_cuda_free(dir.ent);
+    mz_cuda_free(dir.sha_expect);
     if (stats)
         *stats = st;
     return err;

@@ -21,6 +21,9 @@
  *            (the host writer returns MZ_INTERNAL_ERROR for it). A second scan lays the directory out;
  *   emit     one warp per entry, after K8 encrypted the streams in place (AES): local header, salt and verifier, authentication
  *            code, directory record and the public table row; then one thread writes the end records.
+ * The bases lh_base, cd_base, out_base, n_base and the comment place the new entries behind entries already in the archive
+ * (mz_zip_cuda_update_device, zipup_kernel.cuh): local headers (and so the zip64 decision) see absolute offsets, the new records
+ * follow cd_base bytes of kept records, the end records count n_base + n entries. All are 0 or empty for write_device.
  * No CTA waits on another, so the kernels also run on the CPU emulator. Every archive byte is written only below `cap`.
  * The layout rules are those of the host writer, written a second time here on purpose: the host writer serves host-resident
  * entries and is the reference the device output is compared with byte for byte.
@@ -77,6 +80,9 @@ struct ZwCall { /* mirror of mz_cuda_zip_wr */
     unsigned long long *max_csize;
     const uint8_t *digest, *salt, *keys, *mac;
     void *entries;
+    uint64_t lh_base, cd_base, out_base; /* in front of the new entries: archive bytes, directory bytes, output slots */
+    uint32_t n_base, comment_len;         /* entries in front; the end record's comment */
+    const uint8_t *comment;
 };
 
 __device__ __forceinline__ uint32_t zw_salt_len(uint32_t aes) { return aes ? 4 * aes + 4 : 0; }
@@ -154,7 +160,7 @@ __global__ void __launch_bounds__(ZC_THREADS) zw_place_kernel(ZwCall W, uint64_t
         if (j) W.S[c] = run; /* S[c0] is the previous round's: read above by every thread, not written again */
         if (j == m) break;
         const uint32_t len = W.out_len[c], e = W.c_item[c];
-        const uint64_t d = W.pre[e].overhead + zw_head(W, W.items[e].name_len) + run;
+        const uint64_t d = W.lh_base + W.pre[e].overhead + zw_head(W, W.items[e].name_len) + run;
         W.dst[c] = d;
         W.glen[c] = d + len <= W.cap ? len : 0u;
         run += len;
@@ -186,7 +192,7 @@ __global__ void __launch_bounds__(ZW_THREADS) zw_entries_kernel(ZwCall W, const 
     const uint64_t last_len = size - nfull * ZW_CHUNK;
     const uint32_t r = gf2_mulmod(acc, gf2_xpow(cc->x2n, 8 * last_len)) ^ W.residue[last];
     const uint32_t crc = size ? ~(gf2_mulmod(0xffffffffu, gf2_xpow(cc->x2n, 8 * size)) ^ r) : 0u;
-    const uint64_t lh = W.pre[e].overhead + W.S[first], csize = W.S[last + 1] - W.S[first];
+    const uint64_t lh = W.lh_base + W.pre[e].overhead + W.S[first], csize = W.S[last + 1] - W.S[first];
     W.e_lh[e] = lh;
     W.e_csize[e] = csize;
     W.e_crc[e] = crc;
@@ -235,7 +241,7 @@ __global__ void __launch_bounds__(ZW_THREADS) zw_emit_kernel(ZwCall W, uint64_t 
     const uint32_t crc = W.e_crc[e], date = it.dos_date ? it.dos_date : W.dos_now;
     const uint32_t fa = it.external_fa ? it.external_fa : (0100644u << 16);
     const bool z64 = lh >= 0xffffffffull;
-    const uint64_t cd = cd_off + W.e_cdpre[e];
+    const uint64_t cd = cd_off + W.cd_base + W.e_cdpre[e];
     if (lane == 0) {
         o.u32(lh, 0x04034b50u);                           /* local header (za_prepare) */
         o.u16(lh + 4, W.aes ? 51 : 20);
@@ -289,7 +295,7 @@ __global__ void __launch_bounds__(ZW_THREADS) zw_emit_kernel(ZwCall W, uint64_t 
         d.local_off = lh;
         d.csize = stored;
         d.usize = it.size;
-        d.out_off = W.pre[e].out16;
+        d.out_off = W.out_base + W.pre[e].out16;
         d.name_off = cd + 46;
         d.extent = (e + 1 < W.n ? W.e_lh[e + 1] : cd_off) - lh;
         d.sha_off = W.sha ? cd + 46 + nlen + (z64 ? 28 : 0) + (W.aes ? 11 : 0) + 8 : 0;
@@ -304,12 +310,15 @@ __global__ void __launch_bounds__(ZW_THREADS) zw_emit_kernel(ZwCall W, uint64_t 
 }
 
 /* the end records behind the directory (zip64 end record and locator when the directory starts at 0xffffffff or later or there
- * are 0xffff entries or more) */
-__global__ void zw_end_kernel(ZwCall W, uint64_t cd_off, uint64_t cd_size) {
+ * are 0xffff entries or more), written by thread 0; the comment (up to 65535 bytes) by the whole CTA */
+__global__ void __launch_bounds__(ZW_THREADS) zw_end_kernel(ZwCall W, uint64_t cd_off, uint64_t cd_size) {
     const ZwOut o{W.archive, W.cap};
-    const uint64_t n = W.n;
+    const uint64_t n = (uint64_t)W.n_base + W.n;
     uint64_t q = cd_off + cd_size;
-    if (cd_off >= 0xffffffffull || n >= 0xffffu) {
+    const uint64_t z = cd_off >= 0xffffffffull || n >= 0xffffu ? 76 : 0;
+    for (uint32_t k = threadIdx.x; k < W.comment_len; k += ZW_THREADS) o.b(q + z + 22 + k, W.comment[k]);
+    if (threadIdx.x) return;
+    if (z) {
         o.u32(q, 0x06064b50u);
         o.u64(q + 4, 44);
         o.u16(q + 12, (3u << 8) | 45u);
@@ -331,7 +340,7 @@ __global__ void zw_end_kernel(ZwCall W, uint64_t cd_off, uint64_t cd_size) {
     o.u16(q + 10, n >= 0xffffu ? 0xffffu : (uint32_t)n);
     o.u32(q + 12, (uint32_t)cd_size);
     o.u32(q + 16, cd_off >= 0xffffffffull ? 0xffffffffu : (uint32_t)cd_off);
-    o.u16(q + 20, 0);
+    o.u16(q + 20, W.comment_len);
 }
 
 } // namespace mzc
