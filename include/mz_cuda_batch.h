@@ -395,6 +395,75 @@ int32_t mz_cuda_inflate_spec_round(const void *d_in, uint64_t in_base, uint64_t 
                                    uint64_t out_end, void *d_workspace, uint32_t max_segments, mz_cuda_spec_summary *d_summary,
                                    void *stream);
 
+/* ---- gzip members in device memory ------------------------------------------------------------------------------------------
+ * One RFC 1952 member (what the vtbl stream reads and writes with window bits 31, and what minigzip reads and writes) compressed
+ * from a device buffer into a device buffer, and decoded from a device buffer into a device buffer, without the host staging of the
+ * vtbl. Both calls are synchronous on `stream` (NULL = default) and use the current device; device pointers must belong to it. They
+ * never write their input. Each allocates its own scratch, so calls on different streams may run at the same time.
+ *
+ * mz_cuda_gzip_compress_device: d_in[0 .. len) becomes one member at d_out:
+ *     10-byte header | one raw DEFLATE stream of the whole buffer | CRC-32 | ISIZE (len mod 2^32).
+ *   - The header is the vtbl's for the level: MTIME 0, XFL 2 at level 9, 4 at levels 0-1, 0 otherwise, OS 3. level -1 is 6; a level
+ *     outside -1..9 gives MZ_PARAM_ERROR, as do out_len == NULL and d_in == NULL with len > 0.
+ *   - The stream is the vtbl's chunking over the whole buffer: 64 KiB chunks, each with MZ_CUDA_FLAG_DICT, so at levels 6-9 every
+ *     chunk may refer back into the 32 KiB in front of it; only the last chunk is FINAL; an empty input gives 03 00. So at levels 0-5
+ *     the member is byte for byte what mz_stream_cuda_write writes for the same bytes, and at levels 6-9 too when the input fits
+ *     one vtbl batch (MZ_CUDA_BATCH_KB, 32 MiB by default; the vtbl's history restarts at each batch, this call's does not). An input
+ *     that is a whole number of vtbl batches is the exception: the vtbl then closes its stream with an extra empty final block.
+ *   - Rounds of MZ_CUDA_ZIP_ROUND_MB plain bytes (default 1024, at most 2048) bound the slot scratch; the rounds run without host
+ *     synchronisation, and the call synchronises once at its end, for the exact length.
+ *   - d_out == NULL is a sizing call: *out_len = an upper bound of the member's length, nothing runs. Otherwise *out_len = the exact
+ *     length; when it is larger than cap the call returns MZ_BUF_ERROR. No byte at or beyond d_out + cap is ever written.
+ *   - stats (optional): bytes_in = len, bytes_out = the member's length, rounds; header_ms / work_ms (rounds) / crc_ms (CRC and
+ *     trailer) are device times between events on `stream`, setup_ms the scratch allocation.
+ *
+ * mz_cuda_gzip_decompress_device: the member at d_in[0 .. len) decoded into d_out[0 .. cap). The framing rules are the vtbl's read
+ * path's (same bytes, same result):
+ *   - header: bad magic, a method other than 8 or reserved flag bits give MZ_DATA_ERROR, a header cut short MZ_BUF_ERROR (fewer than
+ *     10 bytes with a right or missing magic, or FEXTRA / FNAME / FCOMMENT / FHCRC running past len). FHCRC's two bytes are skipped,
+ *     not verified (as the vtbl does).
+ *   - the raw stream is decoded by K5 and K6 straight into d_out: at every block boundary with at least 4 K6 segments of input ahead a
+ *     K6 round, otherwise K5 up to the next block boundary (MZ_CUDA_SPEC=0: K5 only; MZ_CUDA_SPEC_SEG_KB: the segment size, as for
+ *     the vtbl). A truncated or corrupt stream returns the vtbl's code for it (MZ_DATA_ERROR, MZ_BUF_ERROR).
+ *   - trailer: CRC-32 (K1 over the output) and ISIZE must equal the trailer's (MZ_DATA_ERROR); a trailer cut short gives MZ_BUF_ERROR.
+ *   - output larger than cap: MZ_BUF_ERROR with res->out_full = 1. No byte at or beyond d_out + cap is ever written. d_out may be NULL
+ *     only with cap 0.
+ *   - bytes after the member (a second member, padding) are ignored: only the first member is decoded, as by zlib with window bits 31.
+ *   - res (required): header_len; in_used = header + raw stream + trailer, the vtbl's TOTAL_IN at the end (set when the stream was
+ *     decoded to its end: len itself when the trailer is cut short); out_len and crc of the bytes written; out_full.
+ *   - stats (optional): bytes_in = in_used, bytes_out = out_len, k5_launches, k6_rounds; header_ms (header readback and parse),
+ *     setup_ms (scratch allocation and the copy of the raw stream into it: 4-byte aligned with 64 zero bytes behind it, what K5 and K6
+ *     need whatever the caller's pointer and length), work_ms (K5 / K6), crc_ms (CRC and trailer check): host clocks. */
+typedef struct mz_cuda_gzip_stats {
+    uint64_t bytes_in, bytes_out;
+    uint32_t k5_launches, k6_rounds; /* decode only */
+    uint32_t rounds, pad;            /* encode only: deflate rounds */
+    double header_ms, work_ms, crc_ms, setup_ms;
+} mz_cuda_gzip_stats;
+int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t level, void *d_out, uint64_t cap, uint64_t *out_len,
+                                     mz_cuda_gzip_stats *stats, void *stream);
+
+typedef struct mz_cuda_gzip_result {
+    uint64_t header_len; /* bytes of the gzip header */
+    uint64_t in_used;    /* header + raw stream + 8-byte trailer: what the vtbl reports as TOTAL_IN at the end */
+    uint64_t out_len;    /* plain bytes written to d_out */
+    uint32_t crc;        /* CRC-32 of those bytes */
+    uint32_t out_full;   /* 1: decoding stopped because the output reached cap */
+} mz_cuda_gzip_result;
+int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_out, uint64_t cap, mz_cuda_gzip_result *res,
+                                       mz_cuda_gzip_stats *stats, void *stream);
+
+/* K14 (csrc/gzip_kernel.cuh), the device half of mz_cuda_gzip_compress_device. place: chunks [c0, c0 + m) (m <= 32768) of a round,
+ * d_out_len their K2+K3 stream lengths; d_S[c0] = the stream bytes in front of the round (set by the previous round, 0 before the
+ * first) -> d_S[c0 + 1 .. c0 + m], d_dst[c] = head + d_S[c], d_glen[c] = d_out_len[c], or 0 when the chunk would pass cap: the
+ * arguments of K4 mz_cuda_gather. d_part: scan scratch of m / MZ_CUDA_ZIP_WR_TILE + 1 words. trailer: d_crc[0] (a
+ * mz_cuda_crc32_fold result's second word) and len mod 2^32 to d_out + head + *d_S_end when all 8 bytes lie below cap;
+ * *d_total = head + *d_S_end + 8. */
+int32_t mz_cuda_gzip_place(const uint32_t *d_out_len, uint64_t c0, uint32_t m, uint64_t *d_S, uint64_t *d_dst, uint32_t *d_glen, uint64_t head,
+                           uint64_t cap, uint32_t *d_part, void *stream);
+int32_t mz_cuda_gzip_trailer(const uint64_t *d_S_end, const uint32_t *d_crc, uint64_t len, uint64_t head, void *d_out, uint64_t cap,
+                             uint64_t *d_total, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,6 +70,8 @@ EXPORTS = [
     "mz_cuda_zip_sel_status",
     # include/mz_cuda_batch.h, K13
     "mz_cuda_zip_up_counts", "mz_cuda_zip_up_copy", "mz_cuda_zip_up_records",
+    # include/mz_cuda_batch.h, gzip members in device memory (K14)
+    "mz_cuda_gzip_compress_device", "mz_cuda_gzip_decompress_device", "mz_cuda_gzip_place", "mz_cuda_gzip_trailer",
 ]
 
 # mz_cuda_zip_entry_cb (include/mz_zip_cuda.h): (userdata, filename, data, size, crc32) -> 0 or an error that stops the extraction
@@ -88,6 +90,18 @@ class ZipDevEntry(C.Structure):
     _fields_ = [("local_off", C.c_uint64), ("csize", C.c_uint64), ("usize", C.c_uint64), ("out_off", C.c_uint64), ("name_off", C.c_uint64),
                 ("extent", C.c_uint64), ("sha_off", C.c_uint64), ("crc", C.c_uint32), ("name_len", C.c_uint32), ("method", C.c_uint16),
                 ("aes", C.c_uint8), ("has_sha", C.c_uint8), ("status", C.c_int32)]
+
+
+class GzipStats(C.Structure):
+    """mz_cuda_gzip_stats (include/mz_cuda_batch.h)"""
+    _fields_ = [("bytes_in", C.c_uint64), ("bytes_out", C.c_uint64), ("k5_launches", C.c_uint32), ("k6_rounds", C.c_uint32),
+                ("rounds", C.c_uint32), ("pad", C.c_uint32), ("header_ms", C.c_double), ("work_ms", C.c_double), ("crc_ms", C.c_double),
+                ("setup_ms", C.c_double)]
+
+
+class GzipResult(C.Structure):
+    """mz_cuda_gzip_result (include/mz_cuda_batch.h)"""
+    _fields_ = [("header_len", C.c_uint64), ("in_used", C.c_uint64), ("out_len", C.c_uint64), ("crc", C.c_uint32), ("out_full", C.c_uint32)]
 
 
 class ZipItem(C.Structure):
@@ -213,6 +227,10 @@ def configure(L):
     sig("mz_cuda_zip_sel_fill", i32, [vp, vp])
     sig("mz_cuda_zip_sel_gather", i32, [vp, vp])
     sig("mz_cuda_zip_sel_status", i32, [vp, vp, u32, u32, vp, vp, vp])
+    sig("mz_cuda_gzip_compress_device", i32, [vp, u64, C.c_int16, vp, u64, C.POINTER(u64), vp, vp])
+    sig("mz_cuda_gzip_decompress_device", i32, [vp, u64, vp, u64, vp, vp, vp])
+    sig("mz_cuda_gzip_place", i32, [vp, u64, u32, vp, vp, vp, u64, u64, vp, vp])
+    sig("mz_cuda_gzip_trailer", i32, [vp, vp, u64, u64, vp, u64, vp, vp])
     return L
 
 
@@ -502,6 +520,54 @@ def update_device(archive, keep=None, files=(), level=6, sha256=False, password=
     out = torch.empty(max(1, n.value), dtype=torch.uint8, device=dev)
     check(lib.mz_zip_cuda_update_device(*args, out.data_ptr(), n.value, C.byref(n), None, None, s), "update_device")
     return out[:n.value].clone()
+
+
+def gzip_compress_device(data, level=6):
+    """Compress a CUDA uint8 tensor into one gzip member in device memory (mz_cuda_gzip_compress_device): the member the vtbl stream
+    writes with window bits 31 for the same bytes. level -1 is 6. Returns a CUDA uint8 tensor of exactly the member's length. Raises
+    on any error, as check() does."""
+    import torch
+    lib = load()
+    check(lib.mz_cuda_init(), "mz_cuda_init")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    assert data.is_cuda and data.dtype == torch.uint8 and data.device == dev, "data: a CUDA uint8 tensor on the current device"
+    src = data.contiguous().reshape(-1)
+    ptr, n = (src.data_ptr() if src.numel() else None), src.numel()
+    s = _stream_ptr()
+    size = C.c_uint64(0)
+    check(lib.mz_cuda_gzip_compress_device(ptr, n, level, None, 0, C.byref(size), None, s), "gzip_compress_device")  # sizing: a bound
+    out = torch.empty(size.value, dtype=torch.uint8, device=dev)
+    check(lib.mz_cuda_gzip_compress_device(ptr, n, level, out.data_ptr(), size.value, C.byref(size), None, s), "gzip_compress_device")
+    return out[:size.value].clone()  # the bound-sized buffer is released: the member's own storage is exactly its length
+
+
+def gzip_decompress_device(data, size_hint=None):
+    """Decode the gzip member at the start of a CUDA uint8 tensor into device memory (mz_cuda_gzip_decompress_device); bytes after the
+    member are ignored. size_hint: the output capacity, by default the member's ISIZE (the tensor's last 4 bytes). ISIZE is the size
+    mod 2^32, and bytes may follow the member, so when the output does not fit the call is repeated once with 2^32 bytes more (at most
+    1032 bytes per input byte, DEFLATE's largest expansion). Returns (out, in_used): the plain bytes as a CUDA uint8 tensor and the
+    bytes of the member (header, stream and trailer). Raises on any error, as check() does."""
+    import torch
+    lib = load()
+    check(lib.mz_cuda_init(), "mz_cuda_init")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    assert data.is_cuda and data.dtype == torch.uint8 and data.device == dev, "data: a CUDA uint8 tensor on the current device"
+    src = data.contiguous().reshape(-1)
+    ptr, n = (src.data_ptr() if src.numel() else None), src.numel()
+    if size_hint is None:
+        size_hint = int.from_bytes(bytes(src[-4:].cpu().numpy().tobytes()), "little") if n >= 4 else 0
+    s = _stream_ptr()
+    res = GzipResult()
+    cap = int(size_hint)
+    for attempt in range(2):
+        out = torch.empty(max(1, cap), dtype=torch.uint8, device=dev)
+        err = lib.mz_cuda_gzip_decompress_device(ptr, n, out.data_ptr(), cap, C.byref(res), None, s)
+        if err != MZ_BUF_ERROR or not res.out_full or attempt:
+            break
+        cap = min(cap + (1 << 32), 1032 * n + 64)
+    check(err, "gzip_decompress_device")
+    got = out[:res.out_len]
+    return (got if res.out_len == out.numel() else got.clone()), res.in_used
 
 
 def inflate_device(comp, out_cap):

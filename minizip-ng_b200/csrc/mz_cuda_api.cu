@@ -12,6 +12,7 @@
 #include "concat_kernel.cuh"
 #include "crc32_kernel.cuh"
 #include "deflate_kernel.cuh"
+#include "gzip_kernel.cuh"
 #include <cstdlib>
 #include <cstdio>
 #include "inflate_kernel.cuh"
@@ -951,6 +952,35 @@ int32_t mz_cuda_zip_sel_status(const uint32_t *d_status, const uint32_t *d_selec
     if (!d_status || !d_select || !d_first) return MZ_PARAM_ERROR;
     MZ_LAUNCH(zs_status_kernel, dim3((n + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, (cudaStream_t)stream, d_status, d_select, n, count,
               d_out, (unsigned long long *)d_first);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+/* ---- K14: a gzip member written into device memory ---------------------------------------------------------------- */
+int32_t mz_cuda_gzip_place(const uint32_t *d_out_len, uint64_t c0, uint32_t m, uint64_t *d_S, uint64_t *d_dst, uint32_t *d_glen, uint64_t head,
+                           uint64_t cap, uint32_t *d_part, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!d_out_len || !d_S || !d_dst || !d_glen || !d_part || m > 32768u) return MZ_PARAM_ERROR;
+    if (m == 0) return MZ_OK;
+    const cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t nb = m / ZC_TILE + 1;
+    /* the round's stream bytes fit 32 bits: at most 32768 chunks of mz_cuda_deflate_slot_bound(65536) each */
+    MZ_LAUNCH(zc_scan_reduce_kernel<uint32_t>, dim3(nb), dim3(ZC_THREADS), 0, s, d_out_len + c0, (uint64_t)m, d_part);
+    MZ_LAUNCH(zc_scan_parts_kernel<uint32_t>, dim3(1), dim3(ZC_THREADS), 0, s, d_part, nb);
+    MZ_LAUNCH(gz_place_kernel, dim3(nb), dim3(ZC_THREADS), 0, s, d_out_len, c0, m, (const uint32_t *)d_part, d_S, d_dst, d_glen, head, cap);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+int32_t mz_cuda_gzip_trailer(const uint64_t *d_S_end, const uint32_t *d_crc, uint64_t len, uint64_t head, void *d_out, uint64_t cap,
+                             uint64_t *d_total, void *stream) {
+    DeviceCtx *c;
+    int32_t err = get_ctx(&c);
+    if (err) return err;
+    if (!d_S_end || !d_crc || !d_total || (!d_out && cap)) return MZ_PARAM_ERROR;
+    MZ_LAUNCH(gz_trailer_kernel, dim3(1), dim3(32), 0, (cudaStream_t)stream, d_S_end, d_crc, len, head, (uint8_t *)d_out, cap, d_total);
     CK(cudaGetLastError());
     return MZ_OK;
 }

@@ -506,6 +506,45 @@ int32_t mz_stream_cuda_is_open(void *stream) {
     return MZ_OK;
 }
 
+/* ---- gzip framing, shared by the vtbl and the device-memory calls (mz_cuda_gzip_*_device) ------------------------------------ */
+/* what zlib writes for windowBits 31 (RFC1952): no name, MTIME 0, XFL 2 for level 9, 4 for level < 2, OS 3 */
+static void cu_gzip_header(int lvl, uint8_t h[10]) {
+    static const uint8_t base[10] = {0x1f, 0x8b, 8, 0, 0, 0, 0, 0, 0, 3};
+    memcpy(h, base, 10);
+    h[8] = (uint8_t)(lvl == 9 ? 2 : (lvl < 2 ? 4 : 0));
+}
+
+/* the header at p[0 .. n): *hdr_size = its length; MZ_DATA_ERROR for bad magic, method or flags, MZ_BUF_ERROR when it runs past n */
+static int32_t cu_gzip_parse(const uint8_t *p, size_t n, size_t *hdr_size) {
+    size_t i;
+    if (n < 10)
+        return n >= 2 && (p[0] != 0x1f || p[1] != 0x8b) ? MZ_DATA_ERROR : MZ_BUF_ERROR;
+    if (p[0] != 0x1f || p[1] != 0x8b || p[2] != 8 || (p[3] & 0xe0))
+        return MZ_DATA_ERROR;
+    i = 10;
+    if (p[3] & 4) {
+        if (i + 2 > n)
+            return MZ_BUF_ERROR;
+        i += 2 + ((size_t)p[i] | ((size_t)p[i + 1] << 8));
+    }
+    if (p[3] & 8) {
+        while (i < n && p[i])
+            i++;
+        i++;
+    }
+    if (p[3] & 16) {
+        while (i < n && p[i])
+            i++;
+        i++;
+    }
+    if (p[3] & 2)
+        i += 2;
+    if (i > n)
+        return MZ_BUF_ERROR;
+    *hdr_size = i;
+    return MZ_OK;
+}
+
 /* ---- write side --------------------------------------------------------------------------------------- */
 #ifndef MZ_ZIP_NO_COMPRESSION
 static int32_t cu_emit(mz_stream_cuda *cu, const uint8_t *p, uint64_t n) {
@@ -527,9 +566,8 @@ static int32_t cu_write_header(mz_stream_cuda *cu) {
         return MZ_OK;
     cu->header_done = 1;
     if (cu->wrap == 2) {
-        /* what zlib writes for windowBits 31 (RFC1952): no name, MTIME 0, XFL 2 for level 9, 4 for level < 2, OS 3 */
-        uint8_t h[10] = {0x1f, 0x8b, 8, 0, 0, 0, 0, 0, 0, 3};
-        h[8] = (uint8_t)(lvl == 9 ? 2 : (lvl < 2 ? 4 : 0));
+        uint8_t h[10];
+        cu_gzip_header(lvl, h);
         return cu_emit(cu, h, 10);
     }
     if (cu->wrap == 1) {
@@ -817,30 +855,9 @@ static int32_t cu_parse_header(mz_stream_cuda *cu) {
             return MZ_DATA_ERROR;
         cu->hdr_size = 2;
     } else {
-        if (n < 10)
-            return n >= 2 && (p[0] != 0x1f || p[1] != 0x8b) ? MZ_DATA_ERROR : MZ_BUF_ERROR;
-        if (p[0] != 0x1f || p[1] != 0x8b || p[2] != 8 || (p[3] & 0xe0))
-            return MZ_DATA_ERROR;
-        i = 10;
-        if (p[3] & 4) {
-            if (i + 2 > n)
-                return MZ_BUF_ERROR;
-            i += 2 + ((size_t)p[i] | ((size_t)p[i + 1] << 8));
-        }
-        if (p[3] & 8) {
-            while (i < n && p[i])
-                i++;
-            i++;
-        }
-        if (p[3] & 16) {
-            while (i < n && p[i])
-                i++;
-            i++;
-        }
-        if (p[3] & 2)
-            i += 2;
-        if (i > n)
-            return MZ_BUF_ERROR;
+        const int32_t err = cu_gzip_parse(p, n, &i);
+        if (err != MZ_OK)
+            return err;
         cu->hdr_size = (int64_t)i;
     }
     /* drop the framing: the window starts at raw-stream byte 0 */
@@ -854,14 +871,20 @@ static int32_t cu_parse_header(mz_stream_cuda *cu) {
 
 /* A stream that fills the first (small) compressed window is a long one: switch the workspace to big windows and
  * give it the scratch memory of the segment-speculative decoder (K6). Called before the first byte is decoded. */
-static void ws_read_upgrade(mz_stream_cuda *cu) {
-    cu_ws *w = cu->ws;
+/* the K6 segment size in bytes, 0 when speculative rounds are off (MZ_CUDA_SPEC=0, or MZ_CUDA_SPEC_SEG_KB below 1 KiB) */
+static size_t cu_spec_seg(void) {
     const char *off = getenv("MZ_CUDA_SPEC");
     if (off && off[0] == '0')
-        return;
-    size_t cin_cap = env_size("MZ_CUDA_READ_WINDOW_KB", 128u << 20, 1024);
+        return 0;
     size_t seg = env_size("MZ_CUDA_SPEC_SEG_KB", 16u << 10, 1024);
-    if (cin_cap <= w->cin_cap || seg < 1024)
+    return seg < 1024 ? 0 : seg;
+}
+
+static void ws_read_upgrade(mz_stream_cuda *cu) {
+    cu_ws *w = cu->ws;
+    size_t cin_cap = env_size("MZ_CUDA_READ_WINDOW_KB", 128u << 20, 1024);
+    size_t seg = cu_spec_seg();
+    if (!seg || cin_cap <= w->cin_cap)
         return;
     size_t mult = env_size("MZ_CUDA_READ_OUT_MULT", 4, 1); /* output window = this many compressed windows (tests shrink it) */
     size_t win_cap = 32768 + (mult ? mult : 4) * cin_cap;
@@ -920,11 +943,8 @@ static void ws_read_upgrade(mz_stream_cuda *cu) {
 static int ws_spec_ensure(cu_ws *w) {
     if (w->d_spec)
         return 1;
-    const char *off = getenv("MZ_CUDA_SPEC");
-    if (off && off[0] == '0')
-        return 0;
-    size_t seg = env_size("MZ_CUDA_SPEC_SEG_KB", 16u << 10, 1024);
-    if (seg < 1024)
+    size_t seg = cu_spec_seg();
+    if (!seg)
         return 0;
     uint32_t max_seg = (uint32_t)(w->cin_cap / seg) + 1;
     if (max_seg > 12288)
@@ -1578,4 +1598,297 @@ void mz_stream_cuda_delete(void **stream) {
 /* mz_strm_zlib.c:376-378 */
 void *mz_stream_cuda_get_interface(void) {
     return (void *)&mz_stream_cuda_vtbl;
+}
+
+/* ---- gzip members in device memory (include/mz_cuda_batch.h) ----------------------------------------------------------------
+ * The vtbl's framing without its host staging: the member and the plain bytes both stay in device memory. Compress runs K2+K3, K14
+ * place and K4 per round straight into the caller's buffer, then K1 and the K14 trailer; decompress runs K5 and K6 over the whole
+ * member with the caller's buffer as the one output window, then K1 over the output. */
+static inline double cu_ms(uint64_t t0) { return (double)(now_ns() - t0) / 1e6; }
+
+/* one device allocation carved into n pieces, each 256-byte aligned; NULL on failure */
+static uint8_t *cu_carve(const size_t *sz, void **out[], int n) {
+    size_t total = 0;
+    for (int i = 0; i < n; i++)
+        total += (sz[i] + 255) & ~(size_t)255;
+    uint8_t *p = (uint8_t *)mz_cuda_malloc(total ? total : 256);
+    if (!p)
+        return NULL;
+    size_t o = 0;
+    for (int i = 0; i < n; i++) {
+        *out[i] = p + o;
+        o += (sz[i] + 255) & ~(size_t)255;
+    }
+    return p;
+}
+
+int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t level, void *d_out, uint64_t cap, uint64_t *out_len,
+                                     mz_cuda_gzip_stats *stats, void *stream) {
+    mz_cuda_gzip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    if (!out_len || (!d_in && len))
+        return MZ_PARAM_ERROR;
+    *out_len = 0;
+    if (level == MZ_COMPRESS_LEVEL_DEFAULT)
+        level = 6;
+    if (level < 0 || level > 9)
+        return MZ_PARAM_ERROR;
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_strm_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    const uint64_t nch = len ? (len + CU_CHUNK - 1) / CU_CHUNK : 1, last = len - (nch - 1) * CU_CHUNK;
+    const uint64_t stride = mz_cuda_deflate_slot_bound(CU_CHUNK);
+    if (!d_out) { /* sizing: header, the slot bound of every chunk, trailer */
+        *out_len = 10 + (nch - 1) * stride + mz_cuda_deflate_slot_bound((uint32_t)last) + 8;
+        return MZ_OK;
+    }
+    /* rounds: the knob of mz_zip_cuda_write_device; a round's stream bytes must fit K14 place's 32-bit scan (32768 chunks) */
+    uint64_t R = ((uint64_t)env_size("MZ_CUDA_ZIP_ROUND_MB", 1024, 1) << 20) / CU_CHUNK;
+    if (R < 1)
+        R = 1;
+    if (R > 32768)
+        R = 32768;
+    if (R > nch)
+        R = nch;
+    /* 1. scratch and the chunk table (offsets from d_in, so that every chunk sees the 32 KiB in front of it, across rounds too) */
+    uint64_t t0 = now_ns();
+    uint64_t *c_off = NULL, *S = NULL, *dst = NULL, *total = NULL;
+    uint32_t *c_len = NULL, *olen = NULL, *glen = NULL, *residue = NULL, *crc2 = NULL, *part = NULL;
+    uint8_t *c_flags = NULL, *slots = NULL;
+    const size_t n = (size_t)nch;
+    const size_t sz[12] = {n * 8, n * 4, n, n * 4, n * 4, (n + 1) * 8, n * 8, n * 4, 8, 8, ((size_t)R / MZ_CUDA_ZIP_WR_TILE + 1) * 4, (size_t)R * stride};
+    void **pp[12] = {(void **)&c_off, (void **)&c_len, (void **)&c_flags, (void **)&olen, (void **)&glen, (void **)&S, (void **)&dst,
+                     (void **)&residue, (void **)&crc2, (void **)&total, (void **)&part, (void **)&slots};
+    uint8_t *work = cu_carve(sz, pp, 12);
+    uint8_t *h_tab = (uint8_t *)malloc(n * 13);
+    void *ev[4] = {NULL, NULL, NULL, NULL};
+    int32_t err = work && h_tab ? MZ_OK : MZ_MEM_ERROR;
+    for (int i = 0; i < 4 && !err; i++)
+        if (!(ev[i] = mz_cuda_event_create()))
+            err = MZ_MEM_ERROR;
+    if (!err) {
+        uint64_t *o = (uint64_t *)h_tab;
+        uint32_t *l = (uint32_t *)(h_tab + n * 8);
+        uint8_t *f = h_tab + n * 12;
+        for (size_t c = 0; c < n; c++) {
+            o[c] = (uint64_t)c * CU_CHUNK;
+            l[c] = (uint32_t)(c + 1 < n ? CU_CHUNK : last);
+            f[c] = (uint8_t)(MZ_CUDA_FLAG_DICT | (c + 1 == n ? MZ_CUDA_FLAG_FINAL : 0u));
+        }
+        err = mz_cuda_memcpy_h2d(c_off, o, n * 8, stream);
+        if (!err) err = mz_cuda_memcpy_h2d(c_len, l, n * 4, stream);
+        if (!err) err = mz_cuda_memcpy_h2d(c_flags, f, n, stream);
+        if (!err) err = mz_cuda_memset(S, 0, 8, stream);
+        if (!err) err = mz_cuda_memset(crc2, 0, 8, stream); /* the CRC of an empty input */
+    }
+    st.setup_ms = cu_ms(t0);
+    /* 2. header (the bytes below cap), rounds, CRC-32 and trailer; one readback at the end */
+    if (!err) {
+        uint8_t h[10];
+        cu_gzip_header(level, h);
+        err = mz_cuda_event_record(ev[0], stream);
+        if (!err && cap) err = mz_cuda_memcpy_h2d(d_out, h, cap < 10 ? (size_t)cap : 10, stream);
+        if (!err) err = mz_cuda_event_record(ev[1], stream);
+    }
+    for (uint64_t c0 = 0; !err && c0 < nch; c0 += R) {
+        const uint32_t m = (uint32_t)(nch - c0 < R ? nch - c0 : R);
+        err = mz_cuda_deflate_chunks(d_in, 0, 0, c_off + c0, c_len + c0, c_flags + c0, m, 0, level, slots, stride, olen + c0, stream);
+        if (!err) err = mz_cuda_gzip_place(olen, c0, m, S, dst, glen, 10, cap, part, stream);
+        if (!err) err = mz_cuda_gather(slots, stride, glen + c0, m, dst + c0, d_out, stream);
+        st.rounds++;
+    }
+    if (!err) err = mz_cuda_event_record(ev[2], stream);
+    if (!err && len) err = mz_cuda_crc32_segments(d_in, len, CU_CHUNK, NULL, NULL, (uint32_t)nch, residue, NULL, stream);
+    if (!err && len) err = mz_cuda_crc32_fold(residue, (uint32_t)nch, CU_CHUNK, len, crc2, stream);
+    if (!err) err = mz_cuda_gzip_trailer(S + nch, crc2 + 1, len, 10, d_out, cap, total, stream);
+    if (!err) err = mz_cuda_event_record(ev[3], stream);
+    uint64_t exact = 0;
+    if (!err) err = mz_cuda_memcpy_d2h(&exact, total, 8, stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    if (!err) {
+        st.header_ms = mz_cuda_event_elapsed_ms(ev[0], ev[1]);
+        st.work_ms = mz_cuda_event_elapsed_ms(ev[1], ev[2]);
+        st.crc_ms = mz_cuda_event_elapsed_ms(ev[2], ev[3]);
+        st.bytes_in = len;
+        st.bytes_out = exact;
+        *out_len = exact;
+        if (exact > cap)
+            err = MZ_BUF_ERROR;
+    }
+    mz_cuda_stream_sync(stream); /* (after a failure: nothing of this call is still running when its scratch goes) */
+    for (int i = 0; i < 4; i++)
+        mz_cuda_event_destroy(ev[i]);
+    free(h_tab);
+    mz_cuda_free(work);
+    if (stats)
+        *stats = st;
+    return err;
+}
+
+int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_out, uint64_t cap, mz_cuda_gzip_result *res,
+                                       mz_cuda_gzip_stats *stats, void *stream) {
+    mz_cuda_gzip_stats st;
+    memset(&st, 0, sizeof(st));
+    if (stats)
+        *stats = st;
+    if (!res || (!d_in && len) || (!d_out && cap))
+        return MZ_PARAM_ERROR;
+    memset(res, 0, sizeof(*res));
+    if (mz_cuda_init() != MZ_OK) {
+        fprintf(stderr, "mz_strm_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+        return MZ_SUPPORT_ERROR;
+    }
+    /* 1. the header: 4 KiB, then more while FEXTRA / FNAME / FCOMMENT run past what was read */
+    uint64_t t0 = now_ns();
+    size_t hdr = 0, nh = len < 4096 ? (size_t)len : 4096;
+    uint8_t *h = NULL;
+    int32_t err;
+    for (;;) {
+        uint8_t *h2 = (uint8_t *)realloc(h, nh ? nh : 1);
+        if (!h2) {
+            free(h);
+            return MZ_MEM_ERROR;
+        }
+        h = h2;
+        err = nh ? mz_cuda_memcpy_d2h(h, d_in, nh, stream) : MZ_OK;
+        if (!err) err = mz_cuda_stream_sync(stream);
+        if (!err) err = cu_gzip_parse(h, nh, &hdr);
+        if (err != MZ_BUF_ERROR || nh == len)
+            break;
+        nh = len - nh < nh ? (size_t)len : 2 * nh;
+    }
+    free(h);
+    st.header_ms = cu_ms(t0);
+    if (err) {
+        if (stats)
+            *stats = st;
+        return err;
+    }
+    res->header_len = hdr;
+    /* 2. scratch; the raw stream (and whatever follows it) copied once, 4-byte aligned with 64 zero bytes behind it */
+    t0 = now_ns();
+    const uint64_t avail = len - hdr;
+    const size_t seg = cu_spec_seg();
+    uint32_t max_seg = seg ? (uint32_t)(avail / seg) + 1 : 0;
+    if (max_seg > 12288) /* K6c keeps 16 bytes of shared memory per segment */
+        max_seg = 12288;
+    const uint64_t ncrc = (cap + CU_CHUNK - 1) / CU_CHUNK;
+    uint8_t *stage = NULL;
+    void *spec = NULL;
+    mz_cuda_inflate_job *d_job = NULL;
+    mz_cuda_inflate_state *d_state = NULL;
+    mz_cuda_spec_summary *d_sum = NULL;
+    uint32_t *residue = NULL;
+    const size_t sz[6] = {(size_t)avail + 64, seg ? (size_t)mz_cuda_inflate_spec_workspace_bytes(max_seg) : 0, sizeof(*d_job), sizeof(*d_state),
+                          sizeof(*d_sum), (size_t)(ncrc + 2) * 4};
+    void **pp[6] = {(void **)&stage, &spec, (void **)&d_job, (void **)&d_state, (void **)&d_sum, (void **)&residue};
+    uint8_t *work = cu_carve(sz, pp, 6);
+    err = work ? MZ_OK : MZ_MEM_ERROR;
+    if (!err && avail) err = mz_cuda_memcpy_d2d(stage, (const uint8_t *)d_in + hdr, avail, stream);
+    if (!err) err = mz_cuda_memset(stage + avail, 0, 64, stream);
+    mz_cuda_inflate_state s;
+    memset(&s, 0, sizeof(s));
+    if (!err) err = mz_cuda_memcpy_h2d(d_state, &s, sizeof(s), stream);
+    if (!err) err = mz_cuda_stream_sync(stream);
+    st.setup_ms = cu_ms(t0);
+    /* 3. decode: the vtbl's schedule (cu_decode_more) with the caller's buffer as the only output window */
+    t0 = now_ns();
+    uint64_t resume = 0;
+    double ratio = 4.0;
+    while (!err && s.status == 0) {
+        const int worthwhile = seg && avail * 8 > s.in_bitpos + 8 * 4 * (uint64_t)seg; /* cu_spec_worthwhile */
+        if (worthwhile && s.phase == 0 && s.in_bitpos >= resume) {
+            const uint64_t seg_bits = (uint64_t)seg * 8;
+            uint64_t nseg = (avail * 8 - s.in_bitpos + seg_bits - 1) / seg_bits;
+            const uint64_t fit = (uint64_t)((double)(cap - s.out_pos) / (ratio * 1.25 * (double)seg)) + 1;
+            if (nseg > fit)
+                nseg = fit;
+            if (nseg > max_seg)
+                nseg = max_seg;
+            if (nseg >= 2) {
+                mz_cuda_spec_summary sm;
+                err = mz_cuda_inflate_spec_round(stage, 0, avail, 1, s.in_bitpos, seg, (uint32_t)nseg, d_out, 0, s.out_pos, cap, spec, max_seg, d_sum, stream);
+                if (!err) err = mz_cuda_memcpy_d2h(&sm, d_sum, sizeof(sm), stream);
+                if (!err) err = mz_cuda_stream_sync(stream);
+                st.k6_rounds++;
+                if (err)
+                    break;
+                if (sm.flags || sm.nchain == 0 || (sm.end_bit <= s.in_bitpos && sm.status != 1)) {
+                    resume = sm.candidates <= 1 ? s.in_bitpos + nseg * seg_bits : s.in_bitpos + 1; /* (cu_spec_collect) */
+                } else {
+                    const uint64_t used = (sm.end_bit - s.in_bitpos + 7) >> 3;
+                    if (used > 4096)
+                        ratio = (double)sm.total_out / (double)used < 1.0 ? 1.0 : (double)sm.total_out / (double)used;
+                    s.in_bitpos = sm.end_bit;
+                    s.out_pos += sm.total_out;
+                    s.blocks += sm.blocks;
+                    s.status = sm.status;
+                    s.why = 0;
+                    s.phase = 0;
+                    err = mz_cuda_memcpy_h2d(d_state, &s, sizeof(s), stream);
+                    continue;
+                }
+            }
+        }
+        mz_cuda_inflate_job job;
+        job.d_in = stage;
+        job.in_base = 0;
+        job.in_avail = avail;
+        job.d_out = d_out;
+        job.out_base = 0;
+        job.out_cap = cap;
+        job.in_final = 1;
+        job.flags = worthwhile ? MZ_CUDA_INFLATE_STOP_AT_BLOCK : 0u;
+        err = mz_cuda_memcpy_h2d(d_job, &job, sizeof(job), stream);
+        if (!err) err = mz_cuda_inflate_streams(d_job, d_state, 1, stream);
+        if (!err) err = mz_cuda_memcpy_d2h(&s, d_state, sizeof(s), stream);
+        if (!err) err = mz_cuda_stream_sync(stream);
+        st.k5_launches++;
+        if (!err && s.status == 0 && s.why == 2) {
+            res->out_full = 1;
+            err = MZ_BUF_ERROR;
+        } else if (!err && s.status == 0 && s.why == 1) {
+            err = MZ_BUF_ERROR; /* the decoder wants input that does not exist */
+        }
+    }
+    if (!err && s.status < 0)
+        err = s.status; /* MZ_DATA_ERROR / MZ_BUF_ERROR, zlib-compatible */
+    res->out_len = s.out_pos;
+    st.work_ms = cu_ms(t0);
+    /* 4. the trailer: CRC-32 of the output (K1 in call scratch) and ISIZE */
+    t0 = now_ns();
+    if (!err) {
+        const uint64_t raw = (s.in_bitpos + 7) >> 3, nseg = (s.out_pos + CU_CHUNK - 1) / CU_CHUNK;
+        uint32_t crc2[2] = {0, 0};
+        uint8_t t[8];
+        if (nseg) err = mz_cuda_crc32_segments(d_out, s.out_pos, CU_CHUNK, NULL, NULL, (uint32_t)nseg, residue, NULL, stream);
+        if (!err && nseg) err = mz_cuda_crc32_fold(residue, (uint32_t)nseg, CU_CHUNK, s.out_pos, residue + nseg, stream);
+        if (!err && nseg) err = mz_cuda_memcpy_d2h(crc2, residue + nseg, 8, stream);
+        if (!err && raw + 8 <= avail) err = mz_cuda_memcpy_d2h(t, stage + raw, 8, stream);
+        if (!err) err = mz_cuda_stream_sync(stream);
+        if (!err) {
+            res->crc = crc2[1];
+            if (raw + 8 > avail) { /* the trailer is cut short: TOTAL_IN counts what there is */
+                res->in_used = len;
+                err = MZ_BUF_ERROR;
+            } else {
+                const uint32_t tcrc = t[0] | (t[1] << 8) | (t[2] << 16) | ((uint32_t)t[3] << 24);
+                const uint32_t isz = t[4] | (t[5] << 8) | (t[6] << 16) | ((uint32_t)t[7] << 24);
+                res->in_used = hdr + raw + 8;
+                if (tcrc != res->crc || isz != (uint32_t)s.out_pos)
+                    err = MZ_DATA_ERROR;
+            }
+        }
+    }
+    st.crc_ms = cu_ms(t0);
+    mz_cuda_stream_sync(stream);
+    mz_cuda_free(work);
+    st.bytes_in = res->in_used;
+    st.bytes_out = res->out_len;
+    if (stats)
+        *stats = st;
+    return err;
 }
