@@ -148,6 +148,43 @@ uint32_t gather_grid(uint32_t nchunks, int sm_count) {
     return need < resident ? need : resident;
 }
 
+/* a public call struct (include/mz_cuda_batch.h) as its kernel-side mirror; the layouts are pinned by the static_asserts above */
+template <class K, class P> K mirror(const P *p) {
+    static_assert(sizeof(K) == sizeof(P), "mirror layout");
+    K k;
+    memcpy(&k, p, sizeof(k));
+    return k;
+}
+
+/* part = the exclusive prefix of the per-tile sums of in[0, n) (n / ZC_TILE + 1 tiles) */
+template <typename T> void zc_tiles(const T *in, uint64_t n, T *part, cudaStream_t s) {
+    const uint32_t nb = (uint32_t)(n / ZC_TILE + 1);
+    MZ_LAUNCH(zc_scan_reduce_kernel<T>, dim3(nb), dim3(ZC_THREADS), 0, s, in, n, part);
+    MZ_LAUNCH(zc_scan_parts_kernel<T>, dim3(1), dim3(ZC_THREADS), 0, s, part, nb);
+}
+
+/* out[i] = in[0] + ... + in[i-1] for i = 0..n, with the tiles' sums in part (n / ZC_TILE + 1 of them) */
+template <typename T> int32_t zc_scan(const T *in, uint64_t n, T *out, T *part, cudaStream_t s) {
+    zc_tiles(in, n, part, s);
+    MZ_LAUNCH(zc_scan_apply_kernel<T>, dim3((uint32_t)(n / ZC_TILE + 1)), dim3(ZC_THREADS), 0, s, in, n, (const T *)part, out);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
+/* K11 / K14 place for the round's chunks [c0, c0 + m): the tiles' stream bytes into part, then zc_round_place_kernel */
+template <class Base>
+int32_t round_place(Base base_of, const uint32_t *out_len, uint64_t c0, uint32_t m, uint32_t *part, uint64_t *S, uint64_t *dst, uint32_t *glen,
+                    uint64_t cap, cudaStream_t s) {
+    /* the round's stream bytes fit 32 bits: at most 32768 chunks of mz_cuda_deflate_slot_bound(65536) each */
+    if (m > 32768u) return MZ_PARAM_ERROR;
+    if (m == 0) return MZ_OK;
+    zc_tiles(out_len + c0, (uint64_t)m, part, s);
+    MZ_LAUNCH(zc_round_place_kernel<Base>, dim3(m / ZC_TILE + 1), dim3(ZC_THREADS), 0, s, base_of, out_len, c0, m, (const uint32_t *)part, S, dst,
+              glen, cap);
+    CK(cudaGetLastError());
+    return MZ_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -544,16 +581,11 @@ struct ZcScratch {
     }
 };
 
-/* out[i] = in[0] + ... + in[i-1] for i = 0..n */
+/* zc_scan with the tiles' sums in the parse's scratch */
 template <typename T> int32_t zc_scan(const T *in, uint64_t n, T *out, ZcScratch &w) {
-    const uint64_t nb = n / ZC_TILE + 1;
-    T *part = w.get<T>(nb);
+    T *part = w.get<T>(n / ZC_TILE + 1);
     if (!part) return MZ_MEM_ERROR;
-    MZ_LAUNCH(zc_scan_reduce_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, w.s, in, n, part);
-    MZ_LAUNCH(zc_scan_parts_kernel<T>, dim3(1), dim3(ZC_THREADS), 0, w.s, part, (uint32_t)nb);
-    MZ_LAUNCH(zc_scan_apply_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, w.s, in, n, (const T *)part, out);
-    CK(cudaGetLastError());
-    return MZ_OK;
+    return zc_scan(in, n, out, part, w.s);
 }
 
 int32_t zc_read_summary(ZcSummary *h, const ZcSummary *d, cudaStream_t s) {
@@ -730,35 +762,16 @@ int32_t mz_cuda_zip_statuses(const uint32_t *d_status, uint32_t n, void *d_entri
 }
 
 /* ---- K11: a zip archive written into device memory -------------------------------------------------------------- */
-extern "C++" {
-namespace {
-ZwCall zw_call(const mz_cuda_zip_wr *w) {
-    ZwCall W;
-    memcpy(&W, w, sizeof(W));
-    return W;
-}
-/* out[i] = in[0] + ... + in[i-1] for i = 0..n, with the tiles' sums in part (n / ZC_TILE + 1 of them) */
-template <typename T> int32_t zw_scan(const T *in, uint64_t n, T *out, T *part, cudaStream_t s) {
-    const uint64_t nb = n / ZC_TILE + 1;
-    MZ_LAUNCH(zc_scan_reduce_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, s, in, n, part);
-    MZ_LAUNCH(zc_scan_parts_kernel<T>, dim3(1), dim3(ZC_THREADS), 0, s, part, (uint32_t)nb);
-    MZ_LAUNCH(zc_scan_apply_kernel<T>, dim3((uint32_t)nb), dim3(ZC_THREADS), 0, s, in, n, (const T *)part, out);
-    CK(cudaGetLastError());
-    return MZ_OK;
-}
-} // namespace
-} // extern "C++"
-
 int32_t mz_cuda_zip_wr_items(const mz_cuda_zip_wr *w, uint32_t data_null, uint32_t names_null, void *stream) {
     DeviceCtx *c;
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!w || !w->cnt || !w->pre || !w->part || !w->bad || (w->n && !w->items)) return MZ_PARAM_ERROR;
-    const ZwCall W = zw_call(w);
+    const ZwCall W = mirror<ZwCall>(w);
     const cudaStream_t s = (cudaStream_t)stream;
     if (W.n) MZ_LAUNCH(zw_items_kernel, dim3((W.n + ZW_THREADS - 1) / ZW_THREADS), dim3(ZW_THREADS), 0, s, W, data_null, names_null);
     CK(cudaGetLastError());
-    return zw_scan<ZwCount>(W.cnt, W.n, W.pre, (ZwCount *)W.part, s);
+    return zc_scan<ZwCount>(W.cnt, W.n, W.pre, (ZwCount *)W.part, s);
 }
 
 int32_t mz_cuda_zip_wr_chunks(const mz_cuda_zip_wr *w, void *stream) {
@@ -769,7 +782,7 @@ int32_t mz_cuda_zip_wr_chunks(const mz_cuda_zip_wr *w, void *stream) {
     if (w->nch == 0) return MZ_OK;
     const uint64_t g = (w->nch + ZW_THREADS - 1) / ZW_THREADS;
     if (g > 0x7fffffffull) return MZ_SUPPORT_ERROR;
-    MZ_LAUNCH(zw_chunks_kernel, dim3((uint32_t)g), dim3(ZW_THREADS), 0, (cudaStream_t)stream, zw_call(w));
+    MZ_LAUNCH(zw_chunks_kernel, dim3((uint32_t)g), dim3(ZW_THREADS), 0, (cudaStream_t)stream, mirror<ZwCall>(w));
     CK(cudaGetLastError());
     return MZ_OK;
 }
@@ -778,17 +791,9 @@ int32_t mz_cuda_zip_wr_place(const mz_cuda_zip_wr *w, uint64_t c0, uint32_t m, v
     DeviceCtx *c;
     int32_t err = get_ctx(&c);
     if (err) return err;
-    if (!w || !w->out_len || !w->S || !w->dst || !w->glen || !w->part || m > 32768u || c0 + m > w->nch) return MZ_PARAM_ERROR;
-    if (m == 0) return MZ_OK;
-    const cudaStream_t s = (cudaStream_t)stream;
-    const uint32_t nb = m / ZC_TILE + 1;
-    uint32_t *part = (uint32_t *)w->part;
-    /* the round's stream bytes fit 32 bits: at most 32768 chunks of mz_cuda_deflate_slot_bound(65536) each */
-    MZ_LAUNCH(zc_scan_reduce_kernel<uint32_t>, dim3(nb), dim3(ZC_THREADS), 0, s, (const uint32_t *)w->out_len + c0, (uint64_t)m, part);
-    MZ_LAUNCH(zc_scan_parts_kernel<uint32_t>, dim3(1), dim3(ZC_THREADS), 0, s, part, nb);
-    MZ_LAUNCH(zw_place_kernel, dim3(nb), dim3(ZC_THREADS), 0, s, zw_call(w), c0, m, (const uint32_t *)part);
-    CK(cudaGetLastError());
-    return MZ_OK;
+    if (!w || !w->out_len || !w->S || !w->dst || !w->glen || !w->part || c0 + m > w->nch) return MZ_PARAM_ERROR;
+    const ZwCall W = mirror<ZwCall>(w);
+    return round_place(ZwPlaceBase{W}, W.out_len, c0, m, (uint32_t *)W.part, W.S, W.dst, W.glen, W.cap, (cudaStream_t)stream);
 }
 
 int32_t mz_cuda_zip_wr_entries(const mz_cuda_zip_wr *w, void *stream) {
@@ -796,12 +801,12 @@ int32_t mz_cuda_zip_wr_entries(const mz_cuda_zip_wr *w, void *stream) {
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!w || !w->e_lh || !w->e_csize || !w->e_cd || !w->e_cdpre || !w->e_coff || !w->e_crc || !w->max_csize || !w->residue || !w->S) return MZ_PARAM_ERROR;
-    const ZwCall W = zw_call(w);
+    const ZwCall W = mirror<ZwCall>(w);
     const cudaStream_t s = (cudaStream_t)stream;
     const uint32_t per = ZW_THREADS / 32;
     if (W.n) MZ_LAUNCH(zw_entries_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, (const CrcConsts *)c->d_consts);
     CK(cudaGetLastError());
-    return zw_scan<uint64_t>(W.e_cd, W.n, W.e_cdpre, (uint64_t *)W.part, s);
+    return zc_scan<uint64_t>(W.e_cd, W.n, W.e_cdpre, (uint64_t *)W.part, s);
 }
 
 int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t cd_size, void *stream) {
@@ -809,7 +814,7 @@ int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t c
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!w || !w->archive || (w->sha && !w->digest) || (w->aes && (!w->salt || !w->keys || !w->mac))) return MZ_PARAM_ERROR;
-    const ZwCall W = zw_call(w);
+    const ZwCall W = mirror<ZwCall>(w);
     const cudaStream_t s = (cudaStream_t)stream;
     const uint32_t per = ZW_THREADS / 32;
     if (W.n) MZ_LAUNCH(zw_emit_kernel, dim3((W.n + per - 1) / per), dim3(ZW_THREADS), 0, s, W, cd_off);
@@ -819,27 +824,17 @@ int32_t mz_cuda_zip_wr_emit(const mz_cuda_zip_wr *w, uint64_t cd_off, uint64_t c
 }
 
 /* ---- K13: an archive in device memory updated on the device ------------------------------------------------------ */
-extern "C++" {
-namespace {
-ZuCall zu_call(const mz_cuda_zip_up *u) {
-    ZuCall U;
-    memcpy(&U, u, sizeof(U));
-    return U;
-}
-} // namespace
-} // extern "C++"
-
 int32_t mz_cuda_zip_up_counts(const mz_cuda_zip_up *u, void *stream) {
     DeviceCtx *c;
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!u || !u->cnt || !u->pre || !u->part || !u->info || !u->src || (u->n && (!u->dir || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
-    const ZuCall U = zu_call(u);
+    const ZuCall U = mirror<ZuCall>(u);
     const cudaStream_t s = (cudaStream_t)stream;
     const uint32_t g = (U.n + ZU_THREADS - 1) / ZU_THREADS;
     if (U.n) MZ_LAUNCH(zu_counts_kernel, dim3(g), dim3(ZU_THREADS), 0, s, U);
     CK(cudaGetLastError());
-    if ((err = zw_scan<ZuCount>(U.cnt, U.n, U.pre, (ZuCount *)U.part, s))) return err;
+    if ((err = zc_scan<ZuCount>(U.cnt, U.n, U.pre, (ZuCount *)U.part, s))) return err;
     if (U.n) MZ_LAUNCH(zu_layout_kernel, dim3(g), dim3(ZU_THREADS), 0, s, U);
     MZ_LAUNCH(zu_comment_kernel, dim3(1), dim3(ZU_THREADS), 0, s, U);
     CK(cudaGetLastError());
@@ -853,7 +848,7 @@ int32_t mz_cuda_zip_up_copy(const mz_cuda_zip_up *u, void *stream) {
     if (!u || !u->pre || !u->archive || (u->n && (!u->src || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
     if (u->n == 0) return MZ_OK;
     const uint32_t per = ZU_THREADS / 32, g = (u->n + per - 1) / per, cap = (uint32_t)c->sm_count * 8u;
-    MZ_LAUNCH(zu_copy_kernel, dim3(g < cap ? g : cap), dim3(ZU_THREADS), 0, (cudaStream_t)stream, zu_call(u));
+    MZ_LAUNCH(zu_copy_kernel, dim3(g < cap ? g : cap), dim3(ZU_THREADS), 0, (cudaStream_t)stream, mirror<ZuCall>(u));
     CK(cudaGetLastError());
     return MZ_OK;
 }
@@ -865,7 +860,7 @@ int32_t mz_cuda_zip_up_records(const mz_cuda_zip_up *u, void *stream) {
     if (!u || !u->pre || !u->info || !u->archive || (u->n && (!u->dir || (u->count && !u->ent)))) return MZ_PARAM_ERROR;
     if (u->n == 0) return MZ_OK;
     const uint32_t per = ZU_THREADS / 32;
-    MZ_LAUNCH(zu_records_kernel, dim3((u->n + per - 1) / per), dim3(ZU_THREADS), 0, (cudaStream_t)stream, zu_call(u));
+    MZ_LAUNCH(zu_records_kernel, dim3((u->n + per - 1) / per), dim3(ZU_THREADS), 0, (cudaStream_t)stream, mirror<ZuCall>(u));
     CK(cudaGetLastError());
     return MZ_OK;
 }
@@ -898,26 +893,16 @@ int32_t mz_cuda_zip_name_lookup(const void *d_archive, const void *d_entries, co
     return MZ_OK;
 }
 
-extern "C++" {
-namespace {
-ZsCall zs_call(const mz_cuda_zip_sel *c) {
-    ZsCall C;
-    memcpy(&C, c, sizeof(C));
-    return C;
-}
-} // namespace
-} // extern "C++"
-
 int32_t mz_cuda_zip_sel_counts(const mz_cuda_zip_sel *sc, void *stream) {
     DeviceCtx *c;
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!sc || !sc->cnt || !sc->pre || !sc->part || (sc->n && (!sc->select || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
-    const ZsCall C = zs_call(sc);
+    const ZsCall C = mirror<ZsCall>(sc);
     const cudaStream_t s = (cudaStream_t)stream;
     if (C.n) MZ_LAUNCH(zs_count_kernel, dim3((C.n + ZS_THREADS - 1) / ZS_THREADS), dim3(ZS_THREADS), 0, s, C);
     CK(cudaGetLastError());
-    return zw_scan<ZsCount>(C.cnt, C.n, C.pre, (ZsCount *)C.part, s);
+    return zc_scan<ZsCount>(C.cnt, C.n, C.pre, (ZsCount *)C.part, s);
 }
 
 int32_t mz_cuda_zip_sel_fill(const mz_cuda_zip_sel *sc, void *stream) {
@@ -925,7 +910,7 @@ int32_t mz_cuda_zip_sel_fill(const mz_cuda_zip_sel *sc, void *stream) {
     int32_t err = get_ctx(&c);
     if (err) return err;
     if (!sc || !sc->pre || (sc->sel && sc->n && (!sc->select || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
-    const ZsCall C = zs_call(sc);
+    const ZsCall C = mirror<ZsCall>(sc);
     MZ_LAUNCH(zs_fill_kernel, dim3(C.n / ZS_THREADS + 1), dim3(ZS_THREADS), 0, (cudaStream_t)stream, C);
     CK(cudaGetLastError());
     return MZ_OK;
@@ -938,7 +923,7 @@ int32_t mz_cuda_zip_sel_gather(const mz_cuda_zip_sel *sc, void *stream) {
     if (!sc || !sc->pre || (sc->n && (!sc->select || !sc->archive || !sc->scratch || (sc->count && !sc->ent)))) return MZ_PARAM_ERROR;
     if (sc->n == 0) return MZ_OK;
     const uint32_t per = ZS_THREADS / 32, g = (sc->n + per - 1) / per, cap = (uint32_t)c->sm_count * 8u;
-    MZ_LAUNCH(zs_gather_kernel, dim3(g < cap ? g : cap), dim3(ZS_THREADS), 0, (cudaStream_t)stream, zs_call(sc));
+    MZ_LAUNCH(zs_gather_kernel, dim3(g < cap ? g : cap), dim3(ZS_THREADS), 0, (cudaStream_t)stream, mirror<ZsCall>(sc));
     CK(cudaGetLastError());
     return MZ_OK;
 }
@@ -962,16 +947,8 @@ int32_t mz_cuda_gzip_place(const uint32_t *d_out_len, uint64_t c0, uint32_t m, u
     DeviceCtx *c;
     int32_t err = get_ctx(&c);
     if (err) return err;
-    if (!d_out_len || !d_S || !d_dst || !d_glen || !d_part || m > 32768u) return MZ_PARAM_ERROR;
-    if (m == 0) return MZ_OK;
-    const cudaStream_t s = (cudaStream_t)stream;
-    const uint32_t nb = m / ZC_TILE + 1;
-    /* the round's stream bytes fit 32 bits: at most 32768 chunks of mz_cuda_deflate_slot_bound(65536) each */
-    MZ_LAUNCH(zc_scan_reduce_kernel<uint32_t>, dim3(nb), dim3(ZC_THREADS), 0, s, d_out_len + c0, (uint64_t)m, d_part);
-    MZ_LAUNCH(zc_scan_parts_kernel<uint32_t>, dim3(1), dim3(ZC_THREADS), 0, s, d_part, nb);
-    MZ_LAUNCH(gz_place_kernel, dim3(nb), dim3(ZC_THREADS), 0, s, d_out_len, c0, m, (const uint32_t *)d_part, d_S, d_dst, d_glen, head, cap);
-    CK(cudaGetLastError());
-    return MZ_OK;
+    if (!d_out_len || !d_S || !d_dst || !d_glen || !d_part) return MZ_PARAM_ERROR;
+    return round_place(GzPlaceBase{head}, d_out_len, c0, m, d_part, d_S, d_dst, d_glen, cap, (cudaStream_t)stream);
 }
 
 int32_t mz_cuda_gzip_trailer(const uint64_t *d_S_end, const uint32_t *d_crc, uint64_t len, uint64_t head, void *d_out, uint64_t cap,

@@ -27,6 +27,7 @@
 
 #include "mz_abi.h"
 #include "mz_cuda_batch.h"
+#include "mz_cuda_host.h"
 
 #define CU_CHUNK 65536u
 
@@ -459,11 +460,8 @@ int32_t mz_stream_cuda_open(void *stream, const char *path, int32_t mode) {
         }
 #endif
     }
-    if (mz_cuda_init() != MZ_OK) {
-        cu->error = MZ_SUPPORT_ERROR;
-        fprintf(stderr, "mz_strm_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
-        return MZ_SUPPORT_ERROR;
-    }
+    if (mzh_gpu_required("mz_strm_cuda"))
+        return cu->error = MZ_SUPPORT_ERROR;
     cu->in_len = 0;
     cu->crc = 0;
     cu->crc_bytes = 0;
@@ -1054,13 +1052,50 @@ static int32_t cu_prepare_input(mz_stream_cuda *cu) {
 
 static inline uint8_t *cu_window(const mz_stream_cuda *cu, int which) { return which ? cu->ws->d_win2 : cu->ws->d_win; }
 
-/* enough compressed input ahead of the decoder for a speculative round to pay off: 4 segments (64 KiB). One warp decodes
- * ~13 MB/s of output, so even the two or three zlib blocks of such a window, decoded side by side, beat the serial decoder;
- * below that the round's seven launches cost more than they save. */
+/* ---- the K6 schedule, shared by the vtbl (cu_spec_*) and mz_cuda_gzip_decompress_device ---- */
+/* enough compressed input ahead of the decoder (at bitpos; the input ends at end_bits) for a speculative round to pay off: 4
+ * segments (64 KiB). One warp decodes ~13 MB/s of output, so even the two or three zlib blocks of such a window, decoded side by
+ * side, beat the serial decoder; below that the round's seven launches cost more than they save. */
+static int cu_k6_worthwhile(uint64_t end_bits, uint64_t bitpos, uint64_t seg) {
+    return end_bits > bitpos + 8 * 4 * seg;
+}
+
+/* the next round's segments: the input ahead, but not far more than the output room can take (the running ratio, x 1.25), and at
+ * most max_seg. Fewer than 2: no round. */
+static uint64_t cu_k6_nseg(uint64_t bits_avail, uint64_t room, double ratio, uint64_t seg, uint64_t max_seg) {
+    const uint64_t seg_bits = seg * 8;
+    uint64_t nseg = (bits_avail + seg_bits - 1) / seg_bits;
+    const uint64_t fit = (uint64_t)((double)room / (ratio * 1.25 * (double)seg)) + 1;
+    if (nseg > fit)
+        nseg = fit;
+    if (nseg > max_seg)
+        nseg = max_seg;
+    return nseg;
+}
+
+/* take the summary of a round of nseg segments started at st->in_bitpos. Returns 1 when it proved a chain: st (host copy) and the
+ * running ratio advance. Returns 0 when it proved nothing: the serial decoder moves on, and *resume is where the next round may
+ * start; if the window holds no other block start at all (stored or fixed blocks, one giant block), not before it is consumed. */
+static int cu_k6_take(const mz_cuda_spec_summary *sm, uint64_t nseg, uint64_t seg, mz_cuda_inflate_state *st, double *ratio, uint64_t *resume) {
+    if (sm->flags || sm->nchain == 0 || (sm->end_bit <= st->in_bitpos && sm->status != 1)) {
+        *resume = sm->candidates <= 1 ? st->in_bitpos + nseg * seg * 8 : st->in_bitpos + 1;
+        return 0;
+    }
+    const uint64_t used_bytes = (sm->end_bit - st->in_bitpos + 7) >> 3;
+    if (used_bytes > 4096)
+        *ratio = (double)sm->total_out / (double)used_bytes < 1.0 ? 1.0 : (double)sm->total_out / (double)used_bytes;
+    st->in_bitpos = sm->end_bit;
+    st->out_pos += sm->total_out;
+    st->blocks += sm->blocks;
+    st->status = sm->status;
+    st->why = 0;
+    st->phase = 0;
+    return 1;
+}
+
 static int cu_spec_worthwhile(const mz_stream_cuda *cu) {
     const cu_ws *w = cu->ws;
-    const uint64_t seg = w->spec_seg_bytes ? w->spec_seg_bytes : 16384;
-    return (cu->cin_base + cu->cin_len) * 8 > w->h_state->in_bitpos + 8 * 4 * seg;
+    return cu_k6_worthwhile((cu->cin_base + cu->cin_len) * 8, w->h_state->in_bitpos, w->spec_seg_bytes ? w->spec_seg_bytes : 16384);
 }
 
 static int cu_spec_eligible(mz_stream_cuda *cu) {
@@ -1075,18 +1110,10 @@ static int cu_spec_eligible(mz_stream_cuda *cu) {
 static int32_t cu_spec_launch(mz_stream_cuda *cu) {
     cu_ws *w = cu->ws;
     mz_cuda_inflate_state *st = w->h_state;
-    const uint64_t bits_avail = (cu->cin_base + cu->cin_len) * 8 - st->in_bitpos;
-    const uint64_t seg_bits = (uint64_t)w->spec_seg_bytes * 8;
     const uint64_t out_end = cu->win_base + w->win_cap;
-    const uint64_t room = out_end - st->out_pos;
+    const uint64_t nseg = cu_k6_nseg((cu->cin_base + cu->cin_len) * 8 - st->in_bitpos, out_end - st->out_pos, cu->ratio_est, w->spec_seg_bytes,
+                                     w->spec_max_seg);
     int32_t err;
-    uint64_t nseg = (bits_avail + seg_bits - 1) / seg_bits;
-    /* do not scan far more input than the output window can take (the ratio estimate follows the stream) */
-    uint64_t fit = (uint64_t)((double)room / (cu->ratio_est * 1.25 * (double)w->spec_seg_bytes)) + 1;
-    if (nseg > fit)
-        nseg = fit;
-    if (nseg > w->spec_max_seg)
-        nseg = w->spec_max_seg;
     if (nseg < 2)
         return 0;
     err = mz_cuda_inflate_spec_round(w->d_cin, cu->cin_base, cu->cin_len, cu->base_eof ? 1u : 0u, st->in_bitpos, w->spec_seg_bytes,
@@ -1110,7 +1137,6 @@ static int32_t cu_spec_launch(mz_stream_cuda *cu) {
 static int32_t cu_spec_collect(mz_stream_cuda *cu) {
     cu_ws *w = cu->ws;
     mz_cuda_inflate_state *st = w->h_state;
-    const uint64_t seg_bits = (uint64_t)w->spec_seg_bytes * 8;
     int32_t err;
     CU_TIMED(cu, t_round, err = mz_cuda_event_sync(w->rev));
     cu->n_round += 1;
@@ -1122,21 +1148,8 @@ static int32_t cu_spec_collect(mz_stream_cuda *cu) {
         fprintf(stderr, "mz_strm_cuda: K6 round at bit %llu: %llu segments, %u guesses, %u proven, %llu bytes out, end bit %llu, status %d, flags %u\n",
                 (unsigned long long)st->in_bitpos, (unsigned long long)w->pend_nseg, sm->candidates, sm->nchain, (unsigned long long)sm->total_out,
                 (unsigned long long)sm->end_bit, sm->status, sm->flags);
-    if (sm->flags || sm->nchain == 0 || (sm->end_bit <= st->in_bitpos && sm->status != 1)) {
-        /* nothing proven: let the serial decoder move on; if the window holds no other block start at all
-         * (stored or fixed blocks, one giant block), do not try again before it has been consumed */
-        cu->spec_resume_bit = sm->candidates <= 1 ? st->in_bitpos + w->pend_nseg * seg_bits : st->in_bitpos + 1;
+    if (!cu_k6_take(sm, w->pend_nseg, w->spec_seg_bytes, st, &cu->ratio_est, &cu->spec_resume_bit))
         return 0;
-    }
-    const uint64_t used_bytes = (sm->end_bit - st->in_bitpos + 7) >> 3;
-    if (used_bytes > 4096)
-        cu->ratio_est = (double)sm->total_out / (double)used_bytes < 1.0 ? 1.0 : (double)sm->total_out / (double)used_bytes;
-    st->in_bitpos = sm->end_bit;
-    st->out_pos += sm->total_out;
-    st->blocks += sm->blocks;
-    st->status = sm->status;
-    st->why = 0;
-    st->phase = 0;
     err = mz_cuda_memcpy_h2d(w->d_state, st, sizeof(*st), w->rstream);
     if (err)
         return err;
@@ -1606,22 +1619,6 @@ void *mz_stream_cuda_get_interface(void) {
  * member with the caller's buffer as the one output window, then K1 over the output. */
 static inline double cu_ms(uint64_t t0) { return (double)(now_ns() - t0) / 1e6; }
 
-/* one device allocation carved into n pieces, each 256-byte aligned; NULL on failure */
-static uint8_t *cu_carve(const size_t *sz, void **out[], int n) {
-    size_t total = 0;
-    for (int i = 0; i < n; i++)
-        total += (sz[i] + 255) & ~(size_t)255;
-    uint8_t *p = (uint8_t *)mz_cuda_malloc(total ? total : 256);
-    if (!p)
-        return NULL;
-    size_t o = 0;
-    for (int i = 0; i < n; i++) {
-        *out[i] = p + o;
-        o += (sz[i] + 255) & ~(size_t)255;
-    }
-    return p;
-}
-
 int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t level, void *d_out, uint64_t cap, uint64_t *out_len,
                                      mz_cuda_gzip_stats *stats, void *stream) {
     mz_cuda_gzip_stats st;
@@ -1635,24 +1632,15 @@ int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t lev
         level = 6;
     if (level < 0 || level > 9)
         return MZ_PARAM_ERROR;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_strm_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_strm_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     const uint64_t nch = len ? (len + CU_CHUNK - 1) / CU_CHUNK : 1, last = len - (nch - 1) * CU_CHUNK;
     const uint64_t stride = mz_cuda_deflate_slot_bound(CU_CHUNK);
     if (!d_out) { /* sizing: header, the slot bound of every chunk, trailer */
         *out_len = 10 + (nch - 1) * stride + mz_cuda_deflate_slot_bound((uint32_t)last) + 8;
         return MZ_OK;
     }
-    /* rounds: the knob of mz_zip_cuda_write_device; a round's stream bytes must fit K14 place's 32-bit scan (32768 chunks) */
-    uint64_t R = ((uint64_t)env_size("MZ_CUDA_ZIP_ROUND_MB", 1024, 1) << 20) / CU_CHUNK;
-    if (R < 1)
-        R = 1;
-    if (R > 32768)
-        R = 32768;
-    if (R > nch)
-        R = nch;
+    const uint64_t R = mzh_round_chunks(nch);
     /* 1. scratch and the chunk table (offsets from d_in, so that every chunk sees the 32 KiB in front of it, across rounds too) */
     uint64_t t0 = now_ns();
     uint64_t *c_off = NULL, *S = NULL, *dst = NULL, *total = NULL;
@@ -1662,7 +1650,7 @@ int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t lev
     const size_t sz[12] = {n * 8, n * 4, n, n * 4, n * 4, (n + 1) * 8, n * 8, n * 4, 8, 8, ((size_t)R / MZ_CUDA_ZIP_WR_TILE + 1) * 4, (size_t)R * stride};
     void **pp[12] = {(void **)&c_off, (void **)&c_len, (void **)&c_flags, (void **)&olen, (void **)&glen, (void **)&S, (void **)&dst,
                      (void **)&residue, (void **)&crc2, (void **)&total, (void **)&part, (void **)&slots};
-    uint8_t *work = cu_carve(sz, pp, 12);
+    uint8_t *work = mzh_carve(sz, pp, 12);
     uint8_t *h_tab = (uint8_t *)malloc(n * 13);
     void *ev[4] = {NULL, NULL, NULL, NULL};
     int32_t err = work && h_tab ? MZ_OK : MZ_MEM_ERROR;
@@ -1737,10 +1725,8 @@ int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_o
     if (!res || (!d_in && len) || (!d_out && cap))
         return MZ_PARAM_ERROR;
     memset(res, 0, sizeof(*res));
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_strm_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_strm_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     /* 1. the header: 4 KiB, then more while FEXTRA / FNAME / FCOMMENT run past what was read */
     uint64_t t0 = now_ns();
     size_t hdr = 0, nh = len < 4096 ? (size_t)len : 4096;
@@ -1785,7 +1771,7 @@ int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_o
     const size_t sz[6] = {(size_t)avail + 64, seg ? (size_t)mz_cuda_inflate_spec_workspace_bytes(max_seg) : 0, sizeof(*d_job), sizeof(*d_state),
                           sizeof(*d_sum), (size_t)(ncrc + 2) * 4};
     void **pp[6] = {(void **)&stage, &spec, (void **)&d_job, (void **)&d_state, (void **)&d_sum, (void **)&residue};
-    uint8_t *work = cu_carve(sz, pp, 6);
+    uint8_t *work = mzh_carve(sz, pp, 6);
     err = work ? MZ_OK : MZ_MEM_ERROR;
     if (!err && avail) err = mz_cuda_memcpy_d2d(stage, (const uint8_t *)d_in + hdr, avail, stream);
     if (!err) err = mz_cuda_memset(stage + avail, 0, 64, stream);
@@ -1799,15 +1785,9 @@ int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_o
     uint64_t resume = 0;
     double ratio = 4.0;
     while (!err && s.status == 0) {
-        const int worthwhile = seg && avail * 8 > s.in_bitpos + 8 * 4 * (uint64_t)seg; /* cu_spec_worthwhile */
+        const int worthwhile = seg && cu_k6_worthwhile(avail * 8, s.in_bitpos, seg);
         if (worthwhile && s.phase == 0 && s.in_bitpos >= resume) {
-            const uint64_t seg_bits = (uint64_t)seg * 8;
-            uint64_t nseg = (avail * 8 - s.in_bitpos + seg_bits - 1) / seg_bits;
-            const uint64_t fit = (uint64_t)((double)(cap - s.out_pos) / (ratio * 1.25 * (double)seg)) + 1;
-            if (nseg > fit)
-                nseg = fit;
-            if (nseg > max_seg)
-                nseg = max_seg;
+            const uint64_t nseg = cu_k6_nseg(avail * 8 - s.in_bitpos, cap - s.out_pos, ratio, seg, max_seg);
             if (nseg >= 2) {
                 mz_cuda_spec_summary sm;
                 err = mz_cuda_inflate_spec_round(stage, 0, avail, 1, s.in_bitpos, seg, (uint32_t)nseg, d_out, 0, s.out_pos, cap, spec, max_seg, d_sum, stream);
@@ -1816,18 +1796,7 @@ int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_o
                 st.k6_rounds++;
                 if (err)
                     break;
-                if (sm.flags || sm.nchain == 0 || (sm.end_bit <= s.in_bitpos && sm.status != 1)) {
-                    resume = sm.candidates <= 1 ? s.in_bitpos + nseg * seg_bits : s.in_bitpos + 1; /* (cu_spec_collect) */
-                } else {
-                    const uint64_t used = (sm.end_bit - s.in_bitpos + 7) >> 3;
-                    if (used > 4096)
-                        ratio = (double)sm.total_out / (double)used < 1.0 ? 1.0 : (double)sm.total_out / (double)used;
-                    s.in_bitpos = sm.end_bit;
-                    s.out_pos += sm.total_out;
-                    s.blocks += sm.blocks;
-                    s.status = sm.status;
-                    s.why = 0;
-                    s.phase = 0;
+                if (cu_k6_take(&sm, nseg, seg, &s, &ratio, &resume)) {
                     err = mz_cuda_memcpy_h2d(d_state, &s, sizeof(s), stream);
                     continue;
                 }

@@ -15,6 +15,7 @@
 
 #include "mz_abi.h"
 #include "mz_cuda_batch.h"
+#include "mz_cuda_host.h"
 #include "mz_zip_cuda.h"
 
 #define ZC_CHUNK 65536u
@@ -240,10 +241,8 @@ int32_t mz_zip_cuda_add_buffers_ex(void *zip_handle, const mz_cuda_zip_item *ite
         level = 6;
     if (level < 0 || level > 9)
         return MZ_PARAM_ERROR;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     for (uint32_t i = 0; i < count; i++)
         if (!items[i].filename || items[i].size < 0 || (items[i].size > 0 && !items[i].data))
             return MZ_PARAM_ERROR;
@@ -805,10 +804,8 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
         aes_strength = 3; /* MZ_AES_STRENGTH_256, the reference's default (mz_zip.c:2007-2009) */
     if (aes && (!password || strlen(password) > 128 || aes_strength > 3))
         return MZ_PARAM_ERROR; /* MZ_AES_PW_LENGTH_MAX, mz_strm_wzaes.c:77-79 */
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     /* 64 MiB rounds, four in preparation: each round's entries are packed into pinned staging by its own worker thread (that copy is
      * the slowest stage of a round), and small rounds keep the page-locked allocations -- and the time to make them -- small */
     size_t round_bytes = 64u << 20;
@@ -1420,10 +1417,8 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
         return MZ_SUPPORT_ERROR; /* no zip container in this process */
     if (!zip_handle)
         return MZ_PARAM_ERROR;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     size_t comp_cap = 128u << 20, out_cap = 512u << 20;
     {
         const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
@@ -1805,10 +1800,8 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
     memset(&st, 0, sizeof(st));
     if (!base_stream || (flags & ~MZ_ZIP_CUDA_ALL_DEVICES))
         return MZ_PARAM_ERROR;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     double t0 = now_ms();
     zx_entry *ent = NULL;
     char *names = NULL;
@@ -1974,32 +1967,11 @@ static uint8_t *zd_carve(zr_slot *z, uint32_t n, uint32_t **first) {
     const size_t m = n ? n : 1;
     const size_t sz[17] = {m * 4, m * sizeof(mz_cuda_inflate_job), m * sizeof(mz_cuda_inflate_state), m * 8, m * 8, m * 8, m * 8, m * 8, m * 4,
                            m * 4, m * 4, z->nsha ? m * 32 : 32, m * 16, m * MZ_CUDA_WZAES_KEYREC, 256, m * 20, 4};
-    size_t off[17], total = 0;
-    for (int k = 0; k < 17; k++) {
-        off[k] = total;
-        total += (sz[k] + 255) & ~(size_t)255;
-    }
-    uint8_t *w = (uint8_t *)mz_cuda_malloc(total);
-    if (!w)
-        return NULL;
-    z->d_status = (uint32_t *)(w + off[0]);
-    z->d_job = (mz_cuda_inflate_job *)(w + off[1]);
-    z->d_state = (mz_cuda_inflate_state *)(w + off[2]);
-    z->d_seg_off = (uint64_t *)(w + off[3]);
-    z->d_seg_len64 = (uint64_t *)(w + off[4]);
-    z->d_data_off = (uint64_t *)(w + off[5]);
-    z->d_coff = (uint64_t *)(w + off[6]);
-    z->d_clen = (uint64_t *)(w + off[7]);
-    z->d_seg_len = (uint32_t *)(w + off[8]);
-    z->d_residue = (uint32_t *)(w + off[9]);
-    z->d_crc = (uint32_t *)(w + off[10]);
-    z->d_digest = w + off[11];
-    z->d_salt = w + off[12];
-    z->d_keys = w + off[13];
-    z->d_pw = w + off[14];
-    z->d_mac = w + off[15];
-    *first = (uint32_t *)(w + off[16]);
-    return w;
+    void **out[17] = {(void **)&z->d_status, (void **)&z->d_job, (void **)&z->d_state, (void **)&z->d_seg_off, (void **)&z->d_seg_len64,
+                      (void **)&z->d_data_off, (void **)&z->d_coff, (void **)&z->d_clen, (void **)&z->d_seg_len, (void **)&z->d_residue,
+                      (void **)&z->d_crc, (void **)&z->d_digest, (void **)&z->d_salt, (void **)&z->d_keys, (void **)&z->d_pw, (void **)&z->d_mac,
+                      (void **)first};
+    return mzh_carve(sz, out, 17);
 }
 
 int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
@@ -2012,10 +1984,8 @@ int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const ch
         return MZ_PARAM_ERROR;
     *count = 0;
     *out_bytes = 0;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     const double t0 = now_ms();
     mz_cuda_zip_dir dir;
     memset(&dir, 0, sizeof(dir));
@@ -2097,21 +2067,6 @@ int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const ch
 }
 
 /* ---- an archive written into device memory (mz_zip_cuda_write_device) ---------------------------------------------------- */
-/* carve sizes[k] bytes per piece from one device allocation (256-byte aligned pieces); NULL when it fails */
-static uint8_t *zw_carve(const size_t *sz, void **out[], int k) {
-    size_t off[32], total = 0;
-    for (int i = 0; i < k; i++) {
-        off[i] = total;
-        total += (sz[i] + 255) & ~(size_t)255;
-    }
-    uint8_t *w = (uint8_t *)mz_cuda_malloc(total);
-    if (!w)
-        return NULL;
-    for (int i = 0; i < k; i++)
-        *out[i] = w + off[i];
-    return w;
-}
-
 /* ---- random access to an archive in device memory (mz_zip_cuda_reader_*) ------------------------------------------------- */
 struct mz_zip_cuda_dev_reader {
     int32_t device;
@@ -2166,7 +2121,7 @@ static int32_t zu_reserve(mz_zip_cuda_dev_reader *r, uint32_t n) {
                           (m / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_sel_count), m * sizeof(mz_cuda_zip_ent), 8};
     void **out[5] = {(void **)&r->cnt, (void **)&r->pre, &r->part, (void **)&r->sel, (void **)&r->first};
     if (r->work)
-        r->selw = zw_carve(sz, out, 5);
+        r->selw = mzh_carve(sz, out, 5);
     if (!r->work || !r->selw) {
         mz_cuda_free(r->work);
         r->work = NULL;
@@ -2187,10 +2142,8 @@ int32_t mz_zip_cuda_reader_open(const void *d_archive, uint64_t len, const char 
     *reader = NULL;
     *count = 0;
     *refuse = MZ_OK;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     const double t0 = now_ms();
     mz_cuda_zip_dir dir;
     memset(&dir, 0, sizeof(dir));
@@ -2410,10 +2363,8 @@ static int32_t zw_args(const mz_cuda_zip_dev_item *d_items, uint32_t count, int1
         *aes_strength = 3;
     if ((flags & MZ_ZIP_CUDA_AES) && (!password || strlen(password) > 128 || *aes_strength > 3))
         return MZ_PARAM_ERROR;
-    if (mz_cuda_init() != MZ_OK) {
-        fprintf(stderr, "mz_zip_cuda: no usable sm_90 GPU (%s); there is no CPU fallback\n", mz_cuda_last_error());
+    if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    }
     return MZ_OK;
 }
 
@@ -2459,7 +2410,7 @@ static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_nam
     const size_t sz1[4] = {16, m * sizeof(mz_cuda_zip_wr_count), m * sizeof(mz_cuda_zip_wr_count), tiles * sizeof(mz_cuda_zip_wr_count)};
     void **p1[4] = {(void **)&w.bad, (void **)&w.cnt, (void **)&w.pre, &w.part};
     double ts = now_ms();
-    uint8_t *work1 = zw_carve(sz1, p1, 4), *work2 = NULL;
+    uint8_t *work1 = mzh_carve(sz1, p1, 4), *work2 = NULL;
     st.setup_ms += now_ms() - ts;
     if (!work1) {
         *stats_out = st;
@@ -2490,17 +2441,8 @@ static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_nam
     if (f->before)
         err = f->before(f->ctx, stream);
     /* 2. scratch: the chunk table, a round of slots, per-entry arrays */
-    size_t round_bytes = (size_t)1024 << 20;
-    {
-        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
-        if (v && atoll(v) > 0)
-            round_bytes = (size_t)atoll(v) << 20;
-    }
-    uint64_t R = round_bytes / ZC_CHUNK; /* chunks per round: every chunk holds at most 64 KiB */
-    if (R < 1) R = 1;
-    if (R > 32768) R = 32768;
     w.nch = tot.chunks;
-    if (R > w.nch) R = w.nch ? w.nch : 1;
+    const uint64_t R = mzh_round_chunks(w.nch);
     const uint64_t stride = mz_cuda_deflate_slot_bound(ZC_CHUNK);
     const size_t nch = (size_t)w.nch, n = count ? count : 1;
     const size_t ptiles = ((size_t)R > n ? (size_t)R : n) / MZ_CUDA_ZIP_WR_TILE + 1;
@@ -2517,7 +2459,7 @@ static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_nam
                      (void **)&pw, &spare};
     ts = now_ms();
     if (!err)
-        work2 = zw_carve(sz2, p2, 26);
+        work2 = mzh_carve(sz2, p2, 26);
     st.setup_ms += now_ms() - ts;
     if (!err && !work2)
         err = MZ_MEM_ERROR;
@@ -2709,7 +2651,7 @@ int32_t mz_zip_cuda_update_device(const void *d_src, uint64_t src_len, const uin
                               ((size_t)n / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_up_count), 8 * MZ_CUDA_ZIP_UP_INFO};
         void **p[4] = {(void **)&u->cnt, (void **)&u->pre, &u->part, (void **)&u->info};
         const double ts = now_ms();
-        work = zw_carve(sz, p, 4);
+        work = mzh_carve(sz, p, 4);
         st.setup_ms += now_ms() - ts;
         if (!work)
             err = MZ_MEM_ERROR;

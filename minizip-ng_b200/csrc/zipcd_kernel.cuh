@@ -152,6 +152,35 @@ template <typename T> __global__ void __launch_bounds__(ZC_THREADS) zc_scan_appl
     }
 }
 
+/* ---- round placement (K11 and K14 place): the round's chunks [c0, c0 + m) of a stream cut into chunks --------------------- */
+/* per tile of ZC_TILE chunks, with part[] the exclusive prefix of the tiles' stream bytes (zc_scan_reduce / zc_scan_parts over
+ * out_len + c0): S(c) = S[c0] + the round's bytes in front of c; chunk c goes to base_of(c) + S(c), with copy length 0 when its
+ * bytes would pass cap; S[c0 + m] carries the total into the next round */
+template <class Base>
+__global__ void __launch_bounds__(ZC_THREADS) zc_round_place_kernel(Base base_of, const uint32_t *out_len, uint64_t c0, uint32_t m, const uint32_t *part,
+                                                                    uint64_t *S, uint64_t *dst, uint32_t *glen, uint64_t cap) {
+    __shared__ uint64_t s[ZC_THREADS];
+    const uint64_t base = S[c0];
+    const uint32_t b0 = blockIdx.x * ZC_TILE + threadIdx.x * ZC_ITEMS;
+    uint64_t v = 0;
+    for (uint32_t k = 0; k < ZC_ITEMS; k++)
+        if (b0 + k < m) v += out_len[c0 + b0 + k];
+    uint64_t tot;
+    uint64_t run = base + part[blockIdx.x] + zc_block_scan<uint64_t>(v, s, &tot);
+    for (uint32_t k = 0; k < ZC_ITEMS; k++) {
+        const uint32_t j = b0 + k;
+        if (j > m) break;
+        const uint64_t c = c0 + j;
+        if (j) S[c] = run; /* S[c0] is the previous round's: read above by every thread, not written again */
+        if (j == m) break;
+        const uint32_t len = out_len[c];
+        const uint64_t d = base_of(c) + run;
+        dst[c] = d;
+        glen[c] = d + len <= cap ? len : 0u;
+        run += len;
+    }
+}
+
 /* ---- end records ------------------------------------------------------------------------------------------------- */
 __global__ void __launch_bounds__(ZC_THREADS) zc_end_kernel(const uint8_t *buf, uint64_t len, ZcSummary *S) {
     __shared__ uint64_t red[ZC_THREADS];

@@ -141,31 +141,15 @@ __global__ void __launch_bounds__(ZW_THREADS) zw_chunks_kernel(ZwCall W) {
     }
 }
 
-/* ---- place: the round's chunks [c0, c0 + m) -------------------------------------------------------------------------------- */
-/* per tile of ZC_TILE chunks, with part[] the exclusive prefix of the tiles' stream bytes (zc_scan_reduce / zc_scan_parts over
- * out_len + c0): S(c) = S[c0] + the round's bytes in front of c; S[c0 + m] carries the total into the next round */
-__global__ void __launch_bounds__(ZC_THREADS) zw_place_kernel(ZwCall W, uint64_t c0, uint32_t m, const uint32_t *part) {
-    __shared__ uint64_t s[ZC_THREADS];
-    const uint64_t base = W.S[c0];
-    const uint32_t b0 = blockIdx.x * ZC_TILE + threadIdx.x * ZC_ITEMS;
-    uint64_t v = 0;
-    for (uint32_t k = 0; k < ZC_ITEMS; k++)
-        if (b0 + k < m) v += W.out_len[c0 + b0 + k];
-    uint64_t tot;
-    uint64_t run = base + part[blockIdx.x] + zc_block_scan<uint64_t>(v, s, &tot);
-    for (uint32_t k = 0; k < ZC_ITEMS; k++) {
-        const uint32_t j = b0 + k;
-        if (j > m) break;
-        const uint64_t c = c0 + j;
-        if (j) W.S[c] = run; /* S[c0] is the previous round's: read above by every thread, not written again */
-        if (j == m) break;
-        const uint32_t len = W.out_len[c], e = W.c_item[c];
-        const uint64_t d = W.lh_base + W.pre[e].overhead + zw_head(W, W.items[e].name_len) + run;
-        W.dst[c] = d;
-        W.glen[c] = d + len <= W.cap ? len : 0u;
-        run += len;
+/* ---- place: the round's chunks (zc_round_place_kernel) ------------------------------------------------------------------- */
+/* chunk c's destination in front of S(c): OV(e) and the header of its entry e */
+struct ZwPlaceBase {
+    ZwCall W;
+    __device__ __forceinline__ uint64_t operator()(uint64_t c) const {
+        const uint32_t e = W.c_item[c];
+        return W.lh_base + W.pre[e].overhead + zw_head(W, W.items[e].name_len);
     }
-}
+};
 
 /* ---- entries: one warp per entry ----------------------------------------------------------------------------------------- */
 __global__ void __launch_bounds__(ZW_THREADS) zw_entries_kernel(ZwCall W, const CrcConsts *cc) {
