@@ -104,43 +104,72 @@ static size_t cu_crc_slot_words(size_t batch) {
     return (size_t)((batch / 2 + CU_CRC_SEG - 1) / CU_CRC_SEG) + 8;
 }
 
+/* a write slot's buffers for the workspace's batch into t; returns their number */
+static int ws_slot_pieces(const cu_ws *w, cu_slot *s, mzh_piece *t) {
+    const size_t mc = w->max_chunks, slots = mc * w->slot_stride;
+    int n = 0;
+    t[n++] = MZH_PIN(s->h_in, w->batch);
+    t[n++] = MZH_DEV(s->d_in, w->batch + 64);
+    t[n++] = MZH_DEV(s->d_slots, slots);
+    t[n++] = MZH_DEV(s->d_out, slots);
+    t[n++] = MZH_PIN(s->h_out, slots);
+    t[n++] = MZH_DEV(s->d_out_len, mc * 4);
+    t[n++] = MZH_DEV(s->d_residue, mc * 4);
+    t[n++] = MZH_DEV(s->d_crc2, 8);
+    t[n++] = MZH_DEV(s->d_offsets, (mc + 1) * 8);
+    t[n++] = MZH_PIN(s->h_total, 16);
+    return n;
+}
+
+/* a read workspace's buffers that keep their size: decoded batch, the K5 job and state, the CRC ring's results */
+static int ws_read_pieces(cu_ws *w, mzh_piece *t) {
+    int n = 0;
+    t[n++] = MZH_PIN(w->h_dec, w->batch);
+    t[n++] = MZH_PIN(w->h_job, sizeof(mz_cuda_inflate_job));
+    t[n++] = MZH_DEV(w->d_job, sizeof(mz_cuda_inflate_job));
+    t[n++] = MZH_PIN(w->h_state, sizeof(mz_cuda_inflate_state));
+    t[n++] = MZH_DEV(w->d_state, sizeof(mz_cuda_inflate_state));
+    t[n++] = MZH_DEV(w->d_cres, (size_t)CU_CRC_RING * cu_crc_slot_words(w->batch) * 4);
+    t[n++] = MZH_PIN(w->h_cres, (size_t)CU_CRC_RING * 8);
+    return n;
+}
+
+/* its window set for ring_cap, cin_cap and win_cap (ws_read_upgrade replaces it): the compressed ring (+ 64 zero bytes behind it),
+ * the compressed window on the device, the output window */
+static int ws_win_pieces(cu_ws *w, mzh_piece *t) {
+    t[0] = MZH_PIN(w->h_cin, w->ring_cap + 64);
+    t[1] = MZH_DEV(w->d_cin, w->cin_cap + 64);
+    t[2] = MZH_DEV(w->d_win, w->win_cap + 512);
+    return 3;
+}
+
+/* its K6 set for spec_max_seg segments (made by ws_spec_ensure, replaced by ws_read_upgrade): the scratch, the round's summary */
+static int ws_k6_pieces(cu_ws *w, mzh_piece *t) {
+    t[0] = MZH_DEV(w->d_spec, mz_cuda_inflate_spec_workspace_bytes(w->spec_max_seg));
+    t[1] = MZH_PIN(w->h_sum, sizeof(mz_cuda_spec_summary));
+    t[2] = MZH_DEV(w->d_sum, sizeof(mz_cuda_spec_summary));
+    return 3;
+}
+
 static void ws_destroy(cu_ws *w) {
     if (!w)
         return;
+    mzh_piece t[10];
     for (int i = 0; i < CU_NSLOT; i++) {
         cu_slot *s = &w->slot[i];
-        mz_cuda_host_free(s->h_in);
-        mz_cuda_free(s->d_in);
-        mz_cuda_free(s->d_slots);
-        mz_cuda_free(s->d_out);
-        mz_cuda_host_free(s->h_out);
-        mz_cuda_free(s->d_out_len);
-        mz_cuda_free(s->d_residue);
-        mz_cuda_free(s->d_crc2);
-        mz_cuda_free(s->d_offsets);
-        mz_cuda_host_free(s->h_total);
+        mzh_free(t, ws_slot_pieces(w, s, t));
         mz_cuda_event_destroy(s->ev_h2d);
         mz_cuda_event_destroy(s->ev_d2h[0]);
         mz_cuda_event_destroy(s->ev_d2h[1]);
         mz_cuda_stream_destroy(s->stream);
     }
-    mz_cuda_host_free(w->h_cin);
-    mz_cuda_free(w->d_cin);
-    mz_cuda_free(w->d_win);
+    mzh_free(t, ws_read_pieces(w, t));
+    mzh_free(t, ws_win_pieces(w, t));
+    mzh_free(t, ws_k6_pieces(w, t));
     mz_cuda_free(w->d_win2);
-    mz_cuda_host_free(w->h_dec);
-    mz_cuda_host_free(w->h_job);
-    mz_cuda_free(w->d_job);
-    mz_cuda_host_free(w->h_state);
-    mz_cuda_free(w->d_state);
-    mz_cuda_free(w->d_spec);
-    mz_cuda_host_free(w->h_sum);
-    mz_cuda_free(w->d_sum);
     mz_cuda_event_destroy(w->rev);
     for (int i = 0; i < CU_CRC_RING; i++)
         mz_cuda_event_destroy(w->cev[i]);
-    mz_cuda_free(w->d_cres);
-    mz_cuda_host_free(w->h_cres);
     mz_cuda_stream_destroy(w->rstream);
     mz_cuda_stream_destroy(w->dstream);
     mz_cuda_stream_destroy(w->cstream);
@@ -169,28 +198,17 @@ static cu_ws *ws_acquire(int kind) {
     w->kind = kind;
     w->batch = batch;
     w->device = device;
+    mzh_piece t[10];
     if (kind == 1) {
         w->max_chunks = (uint32_t)(batch / CU_CHUNK);
         w->slot_stride = mz_cuda_deflate_slot_bound(CU_CHUNK);
-        size_t slots = (size_t)w->max_chunks * w->slot_stride;
         for (int i = 0; i < CU_NSLOT; i++) {
             cu_slot *s = &w->slot[i];
             s->stream = mz_cuda_stream_create();
             s->ev_h2d = mz_cuda_event_create();
             s->ev_d2h[0] = mz_cuda_event_create();
             s->ev_d2h[1] = mz_cuda_event_create();
-            s->h_in = (uint8_t *)mz_cuda_host_alloc(batch);
-            s->d_in = (uint8_t *)mz_cuda_malloc(batch + 64);
-            s->d_slots = (uint8_t *)mz_cuda_malloc(slots);
-            s->d_out = (uint8_t *)mz_cuda_malloc(slots);
-            s->h_out = (uint8_t *)mz_cuda_host_alloc(slots);
-            s->d_out_len = (uint32_t *)mz_cuda_malloc((size_t)w->max_chunks * 4);
-            s->d_residue = (uint32_t *)mz_cuda_malloc((size_t)w->max_chunks * 4);
-            s->d_crc2 = (uint32_t *)mz_cuda_malloc(8);
-            s->d_offsets = (uint64_t *)mz_cuda_malloc(((size_t)w->max_chunks + 1) * 8);
-            s->h_total = (uint64_t *)mz_cuda_host_alloc(16);
-            if (!s->stream || !s->ev_h2d || !s->ev_d2h[0] || !s->ev_d2h[1] || !s->h_in || !s->d_in || !s->d_slots || !s->d_out || !s->h_out || !s->d_out_len ||
-                !s->d_residue || !s->d_crc2 || !s->d_offsets || !s->h_total) {
+            if (!s->stream || !s->ev_h2d || !s->ev_d2h[0] || !s->ev_d2h[1] || !mzh_alloc(t, ws_slot_pieces(w, s, t))) {
                 ws_destroy(w);
                 return NULL;
             }
@@ -199,29 +217,20 @@ static cu_ws *ws_acquire(int kind) {
         w->cin_cap = batch / 4 > (1u << 20) ? batch / 4 : (1u << 20);
         w->win_cap = 32768 + batch;
         w->ring_cap = w->cin_cap;
-        w->h_cin = (uint8_t *)mz_cuda_host_alloc(w->ring_cap + 64);
-        if (w->h_cin)
+        const int win_ok = mzh_alloc(t, ws_win_pieces(w, t));
+        if (win_ok)
             memset(w->h_cin + w->ring_cap, 0, 64); /* the pad uploaded behind the window; never written again */
-        w->d_cin = (uint8_t *)mz_cuda_malloc(w->cin_cap + 64);
-        w->d_win = (uint8_t *)mz_cuda_malloc(w->win_cap + 512);
-        w->h_dec = (uint8_t *)mz_cuda_host_alloc(batch);
-        w->h_job = (mz_cuda_inflate_job *)mz_cuda_host_alloc(sizeof(mz_cuda_inflate_job));
-        w->d_job = (mz_cuda_inflate_job *)mz_cuda_malloc(sizeof(mz_cuda_inflate_job));
-        w->h_state = (mz_cuda_inflate_state *)mz_cuda_host_alloc(sizeof(mz_cuda_inflate_state));
-        w->d_state = (mz_cuda_inflate_state *)mz_cuda_malloc(sizeof(mz_cuda_inflate_state));
+        const int read_ok = win_ok && mzh_alloc(t, ws_read_pieces(w, t));
         w->rstream = mz_cuda_stream_create();
         w->dstream = mz_cuda_stream_create();
         w->rev = mz_cuda_event_create();
         w->cstream = mz_cuda_stream_create();
-        w->d_cres = (uint32_t *)mz_cuda_malloc((size_t)CU_CRC_RING * cu_crc_slot_words(batch) * 4);
-        w->h_cres = (uint32_t *)mz_cuda_host_alloc((size_t)CU_CRC_RING * 8);
         int cev_ok = 1;
         for (int i = 0; i < CU_CRC_RING; i++) {
             w->cev[i] = mz_cuda_event_create();
             cev_ok &= w->cev[i] != NULL;
         }
-        if (!cev_ok || !w->cstream || !w->d_cres || !w->h_cres || !w->h_cin || !w->d_cin || !w->d_win || !w->h_dec || !w->h_job || !w->d_job || !w->h_state || !w->d_state || !w->rstream ||
-            !w->dstream || !w->rev) {
+        if (!cev_ok || !read_ok || !w->cstream || !w->rstream || !w->dstream || !w->rev) {
             ws_destroy(w);
             return NULL;
         }
@@ -885,55 +894,36 @@ static void ws_read_upgrade(mz_stream_cuda *cu) {
     if (!seg || cin_cap <= w->cin_cap)
         return;
     size_t mult = env_size("MZ_CUDA_READ_OUT_MULT", 4, 1); /* output window = this many compressed windows (tests shrink it) */
-    size_t win_cap = 32768 + (mult ? mult : 4) * cin_cap;
-    uint32_t max_seg = (uint32_t)(cin_cap / seg) + 1;
-    if (max_seg > 12288) /* K6c keeps 16 bytes of shared memory per segment */
-        max_seg = 12288;
-    const size_t ring_cap = 2 * cin_cap; /* window + as much again read ahead while a round is in flight */
-    uint8_t *h_cin = (uint8_t *)mz_cuda_host_alloc(ring_cap + 64);
-    uint8_t *d_cin = (uint8_t *)mz_cuda_malloc(cin_cap + 64);
-    uint8_t *d_win = (uint8_t *)mz_cuda_malloc(win_cap + 512);
-    uint8_t *d_win2 = (uint8_t *)mz_cuda_malloc(win_cap + 512); /* (optional: without it rounds simply wait for the delivery) */
-    void *d_spec = mz_cuda_malloc((size_t)mz_cuda_inflate_spec_workspace_bytes(max_seg));
-    mz_cuda_spec_summary *h_sum = (mz_cuda_spec_summary *)mz_cuda_host_alloc(sizeof(mz_cuda_spec_summary));
-    mz_cuda_spec_summary *d_sum = (mz_cuda_spec_summary *)mz_cuda_malloc(sizeof(mz_cuda_spec_summary));
-    if (!h_cin || !d_cin || !d_win || !d_spec || !h_sum || !d_sum) { /* stay small */
-        mz_cuda_host_free(h_cin);
-        mz_cuda_free(d_cin);
-        mz_cuda_free(d_win);
-        mz_cuda_free(d_win2);
-        mz_cuda_free(d_spec);
-        mz_cuda_host_free(h_sum);
-        mz_cuda_free(d_sum);
+    /* the large sets are made on a copy of the workspace: if one fails the stream stays small, else they replace the small ones */
+    cu_ws big = *w;
+    big.cin_cap = cin_cap;
+    big.win_cap = 32768 + (mult ? mult : 4) * cin_cap;
+    big.ring_cap = 2 * cin_cap; /* window + as much again read ahead while a round is in flight */
+    big.spec_max_seg = (uint32_t)(cin_cap / seg) + 1;
+    if (big.spec_max_seg > 12288) /* K6c keeps 16 bytes of shared memory per segment */
+        big.spec_max_seg = 12288;
+    big.spec_seg_bytes = seg;
+    big.large = 1;
+    mzh_piece win[3], k6[3];
+    if (!mzh_alloc(win, ws_win_pieces(&big, win)))
+        return;
+    big.d_win2 = (uint8_t *)mz_cuda_malloc(big.win_cap + 512); /* (optional: without it rounds simply wait for the delivery) */
+    if (!mzh_alloc(k6, ws_k6_pieces(&big, k6))) {
+        mzh_free(win, 3);
+        mz_cuda_free(big.d_win2);
         return;
     }
     {
         const size_t n = cu->cin_len + cu->ahead_len, n1 = n < w->ring_cap - cu->cin_off ? n : w->ring_cap - cu->cin_off;
-        memcpy(h_cin, w->h_cin + cu->cin_off, n1);
-        memcpy(h_cin + n1, w->h_cin, n - n1);
-        memset(h_cin + ring_cap, 0, 64);
+        memcpy(big.h_cin, w->h_cin + cu->cin_off, n1);
+        memcpy(big.h_cin + n1, w->h_cin, n - n1);
+        memset(big.h_cin + big.ring_cap, 0, 64);
         cu->cin_off = 0;
     }
-    mz_cuda_host_free(w->h_cin);
-    mz_cuda_free(w->d_cin);
-    mz_cuda_free(w->d_win);
-    mz_cuda_free(w->d_spec); /* the small-window K6 scratch, if a medium stream used this workspace before */
-    mz_cuda_host_free(w->h_sum);
-    mz_cuda_free(w->d_sum);
-    w->h_cin = h_cin;
-    w->d_cin = d_cin;
-    w->d_win = d_win;
+    mzh_free(win, ws_win_pieces(w, win));
+    mzh_free(k6, ws_k6_pieces(w, k6)); /* the small-window K6 scratch, if a medium stream used this workspace before */
     mz_cuda_free(w->d_win2);
-    w->d_win2 = d_win2;
-    w->cin_cap = cin_cap;
-    w->ring_cap = ring_cap;
-    w->win_cap = win_cap;
-    w->d_spec = d_spec;
-    w->spec_max_seg = max_seg;
-    w->spec_seg_bytes = seg;
-    w->h_sum = h_sum;
-    w->d_sum = d_sum;
-    w->large = 1;
+    *w = big;
 }
 
 /* K6 scratch for the current (small) windows: medium streams -- a zip entry of a few megabytes -- are decoded by
@@ -947,19 +937,13 @@ static int ws_spec_ensure(cu_ws *w) {
     uint32_t max_seg = (uint32_t)(w->cin_cap / seg) + 1;
     if (max_seg > 12288)
         max_seg = 12288;
-    w->d_spec = mz_cuda_malloc((size_t)mz_cuda_inflate_spec_workspace_bytes(max_seg));
-    w->h_sum = (mz_cuda_spec_summary *)mz_cuda_host_alloc(sizeof(mz_cuda_spec_summary));
-    w->d_sum = (mz_cuda_spec_summary *)mz_cuda_malloc(sizeof(mz_cuda_spec_summary));
-    if (!w->d_spec || !w->h_sum || !w->d_sum) {
-        mz_cuda_free(w->d_spec);
-        mz_cuda_host_free(w->h_sum);
-        mz_cuda_free(w->d_sum);
-        w->d_spec = NULL;
-        w->h_sum = NULL;
-        w->d_sum = NULL;
+    const uint32_t prev = w->spec_max_seg;
+    mzh_piece t[3];
+    w->spec_max_seg = max_seg;
+    if (!mzh_alloc(t, ws_k6_pieces(w, t))) {
+        w->spec_max_seg = prev;
         return 0;
     }
-    w->spec_max_seg = max_seg;
     w->spec_seg_bytes = seg;
     return 1;
 }
@@ -1647,10 +1631,11 @@ int32_t mz_cuda_gzip_compress_device(const void *d_in, uint64_t len, int16_t lev
     uint32_t *c_len = NULL, *olen = NULL, *glen = NULL, *residue = NULL, *crc2 = NULL, *part = NULL;
     uint8_t *c_flags = NULL, *slots = NULL;
     const size_t n = (size_t)nch;
-    const size_t sz[12] = {n * 8, n * 4, n, n * 4, n * 4, (n + 1) * 8, n * 8, n * 4, 8, 8, ((size_t)R / MZ_CUDA_ZIP_WR_TILE + 1) * 4, (size_t)R * stride};
-    void **pp[12] = {(void **)&c_off, (void **)&c_len, (void **)&c_flags, (void **)&olen, (void **)&glen, (void **)&S, (void **)&dst,
-                     (void **)&residue, (void **)&crc2, (void **)&total, (void **)&part, (void **)&slots};
-    uint8_t *work = mzh_carve(sz, pp, 12);
+    const mzh_piece t[12] = {MZH_DEV(c_off, n * 8), MZH_DEV(c_len, n * 4), MZH_DEV(c_flags, n), MZH_DEV(olen, n * 4),
+                             MZH_DEV(glen, n * 4), MZH_DEV(S, (n + 1) * 8), MZH_DEV(dst, n * 8), MZH_DEV(residue, n * 4),
+                             MZH_DEV(crc2, 8), MZH_DEV(total, 8), MZH_DEV(part, ((size_t)R / MZ_CUDA_ZIP_WR_TILE + 1) * 4),
+                             MZH_DEV(slots, (size_t)R * stride)};
+    uint8_t *work = mzh_carve(t, 12);
     uint8_t *h_tab = (uint8_t *)malloc(n * 13);
     void *ev[4] = {NULL, NULL, NULL, NULL};
     int32_t err = work && h_tab ? MZ_OK : MZ_MEM_ERROR;
@@ -1768,10 +1753,10 @@ int32_t mz_cuda_gzip_decompress_device(const void *d_in, uint64_t len, void *d_o
     mz_cuda_inflate_state *d_state = NULL;
     mz_cuda_spec_summary *d_sum = NULL;
     uint32_t *residue = NULL;
-    const size_t sz[6] = {(size_t)avail + 64, seg ? (size_t)mz_cuda_inflate_spec_workspace_bytes(max_seg) : 0, sizeof(*d_job), sizeof(*d_state),
-                          sizeof(*d_sum), (size_t)(ncrc + 2) * 4};
-    void **pp[6] = {(void **)&stage, &spec, (void **)&d_job, (void **)&d_state, (void **)&d_sum, (void **)&residue};
-    uint8_t *work = mzh_carve(sz, pp, 6);
+    const mzh_piece t[6] = {MZH_DEV(stage, avail + 64), MZH_DEV(spec, seg ? mz_cuda_inflate_spec_workspace_bytes(max_seg) : 0),
+                            MZH_DEV(d_job, sizeof(*d_job)), MZH_DEV(d_state, sizeof(*d_state)), MZH_DEV(d_sum, sizeof(*d_sum)),
+                            MZH_DEV(residue, (ncrc + 2) * 4)};
+    uint8_t *work = mzh_carve(t, 6);
     err = work ? MZ_OK : MZ_MEM_ERROR;
     if (!err && avail) err = mz_cuda_memcpy_d2d(stage, (const uint8_t *)d_in + hdr, avail, stream);
     if (!err) err = mz_cuda_memset(stage + avail, 0, 64, stream);

@@ -75,6 +75,7 @@ static double now_ms(void) {
 typedef struct zc_bufs_s {
     size_t round_bytes;
     uint32_t max_chunks;
+    int with_join; /* d_out / h_out exist (the native writer assembles its own region instead) */
     uint64_t stride;
     uint8_t *h_in, *d_in, *d_slots, *d_out, *h_out;
     uint64_t *h_off, *d_off, *d_joined_off, *h_joined_off;
@@ -84,69 +85,51 @@ typedef struct zc_bufs_s {
     uint8_t *d_digest, *h_digest;                 /* per entry: 32 bytes */
 } zc_bufs;
 
+#define ZC_PIECES 23
+/* b's buffers for its capacities into t; returns their number */
+static int zc_pieces(zc_bufs *b, mzh_piece *t) {
+    const size_t mc = b->max_chunks, join = b->with_join ? mc * b->stride : 0;
+    int n = 0;
+    t[n++] = MZH_PIN(b->h_in, b->round_bytes + 64);
+    t[n++] = MZH_DEV(b->d_in, b->round_bytes + 64);
+    t[n++] = MZH_DEV(b->d_slots, mc * b->stride);
+    t[n++] = MZH_DEV(b->d_out, join);
+    t[n++] = MZH_PIN(b->h_out, join);
+    t[n++] = MZH_PIN(b->h_off, mc * 8);
+    t[n++] = MZH_DEV(b->d_off, mc * 8);
+    t[n++] = MZH_DEV(b->d_joined_off, (mc + 1) * 8);
+    t[n++] = MZH_PIN(b->h_joined_off, (mc + 1) * 8);
+    t[n++] = MZH_PIN(b->h_len, mc * 4);
+    t[n++] = MZH_DEV(b->d_len, mc * 4);
+    t[n++] = MZH_DEV(b->d_out_len, mc * 4);
+    t[n++] = MZH_DEV(b->d_residue, mc * 4);
+    t[n++] = MZH_DEV(b->d_crc, mc * 4);
+    t[n++] = MZH_PIN(b->h_crc, mc * 4);
+    t[n++] = MZH_PIN(b->h_flags, mc);
+    t[n++] = MZH_DEV(b->d_flags, mc);
+    t[n++] = MZH_PIN(b->h_eoff, mc * 8); /* an entry has at least one chunk */
+    t[n++] = MZH_DEV(b->d_eoff, mc * 8);
+    t[n++] = MZH_PIN(b->h_elen, mc * 8);
+    t[n++] = MZH_DEV(b->d_elen, mc * 8);
+    t[n++] = MZH_DEV(b->d_digest, mc * 32);
+    t[n++] = MZH_PIN(b->h_digest, mc * 32);
+    return n;
+}
+
 static void zc_free(zc_bufs *b) {
-    mz_cuda_host_free(b->h_in);
-    mz_cuda_free(b->d_in);
-    mz_cuda_free(b->d_slots);
-    mz_cuda_free(b->d_out);
-    mz_cuda_host_free(b->h_out);
-    mz_cuda_host_free(b->h_off);
-    mz_cuda_free(b->d_off);
-    mz_cuda_free(b->d_joined_off);
-    mz_cuda_host_free(b->h_joined_off);
-    mz_cuda_host_free(b->h_len);
-    mz_cuda_free(b->d_len);
-    mz_cuda_free(b->d_out_len);
-    mz_cuda_free(b->d_residue);
-    mz_cuda_free(b->d_crc);
-    mz_cuda_host_free(b->h_crc);
-    mz_cuda_host_free(b->h_flags);
-    mz_cuda_free(b->d_flags);
-    mz_cuda_host_free(b->h_eoff);
-    mz_cuda_free(b->d_eoff);
-    mz_cuda_host_free(b->h_elen);
-    mz_cuda_free(b->d_elen);
-    mz_cuda_free(b->d_digest);
-    mz_cuda_host_free(b->h_digest);
+    mzh_piece t[ZC_PIECES];
+    mzh_free(t, zc_pieces(b, t));
     memset(b, 0, sizeof(*b));
 }
 
 static int zc_alloc(zc_bufs *b, size_t round_bytes, uint32_t max_chunks, int with_join) {
+    mzh_piece t[ZC_PIECES];
     memset(b, 0, sizeof(*b));
     b->round_bytes = round_bytes;
     b->max_chunks = max_chunks;
+    b->with_join = with_join;
     b->stride = mz_cuda_deflate_slot_bound(ZC_CHUNK);
-    const size_t slots = (size_t)max_chunks * b->stride;
-    b->h_in = (uint8_t *)mz_cuda_host_alloc(round_bytes + 64);
-    b->d_in = (uint8_t *)mz_cuda_malloc(round_bytes + 64);
-    b->d_slots = (uint8_t *)mz_cuda_malloc(slots);
-    b->d_out = with_join ? (uint8_t *)mz_cuda_malloc(slots) : NULL; /* (the native writer assembles its own region instead) */
-    b->h_out = with_join ? (uint8_t *)mz_cuda_host_alloc(slots) : NULL;
-    b->h_off = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-    b->d_off = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-    b->d_joined_off = (uint64_t *)mz_cuda_malloc(((size_t)max_chunks + 1) * 8);
-    b->h_joined_off = (uint64_t *)mz_cuda_host_alloc(((size_t)max_chunks + 1) * 8);
-    b->h_len = (uint32_t *)mz_cuda_host_alloc((size_t)max_chunks * 4);
-    b->d_len = (uint32_t *)mz_cuda_malloc((size_t)max_chunks * 4);
-    b->d_out_len = (uint32_t *)mz_cuda_malloc((size_t)max_chunks * 4);
-    b->d_residue = (uint32_t *)mz_cuda_malloc((size_t)max_chunks * 4);
-    b->d_crc = (uint32_t *)mz_cuda_malloc((size_t)max_chunks * 4);
-    b->h_crc = (uint32_t *)mz_cuda_host_alloc((size_t)max_chunks * 4);
-    b->h_flags = (uint8_t *)mz_cuda_host_alloc(max_chunks);
-    b->d_flags = (uint8_t *)mz_cuda_malloc(max_chunks);
-    b->h_eoff = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8); /* an entry has at least one chunk */
-    b->d_eoff = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-    b->h_elen = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-    b->d_elen = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-    b->d_digest = (uint8_t *)mz_cuda_malloc((size_t)max_chunks * 32);
-    b->h_digest = (uint8_t *)mz_cuda_host_alloc((size_t)max_chunks * 32);
-    if (!b->h_in || !b->d_in || !b->d_slots || (with_join && (!b->d_out || !b->h_out)) || !b->h_off || !b->d_off || !b->d_joined_off || !b->h_joined_off ||
-        !b->h_len || !b->d_len || !b->d_out_len || !b->d_residue || !b->d_crc || !b->h_crc || !b->h_flags || !b->d_flags || !b->h_eoff ||
-        !b->d_eoff || !b->h_elen || !b->d_elen || !b->d_digest || !b->h_digest) {
-        zc_free(b);
-        return 0;
-    }
-    return 1;
+    return mzh_alloc(t, zc_pieces(b, t));
 }
 
 static uint32_t chunks_of(int64_t size) {
@@ -251,12 +234,7 @@ int32_t mz_zip_cuda_add_buffers_ex(void *zip_handle, const mz_cuda_zip_item *ite
             *stats = st;
         return MZ_OK;
     }
-    size_t round_bytes = 256u << 20;
-    {
-        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
-        if (v && atoll(v) > 0)
-            round_bytes = (size_t)atoll(v) << 20;
-    }
+    size_t round_bytes = mzh_round_bytes(256);
     /* an entry is never split over rounds: the round must hold the largest one */
     for (uint32_t i = 0; i < count; i++)
         if ((size_t)items[i].size + 16 > round_bytes)
@@ -436,152 +414,254 @@ static uint32_t za_dos_date(int64_t t) {
     return last_v;
 }
 
+#define ZA_PIECES (ZC_PIECES + 22)
+/* z's buffers for its capacities into t (zc_bufs' first); the WinZip AES ones have no bytes without has_aes */
+static int za_pieces(za_slot *z, mzh_piece *t) {
+    const size_t mc = z->b.max_chunks, aes = z->has_aes ? 1 : 0;
+    int n = zc_pieces(&z->b, t);
+    t[n++] = MZH_PIN(z->h_out_len, mc * 4);
+    t[n++] = MZH_PIN(z->h_dst_off, mc * 8);
+    t[n++] = MZH_DEV(z->d_dst_off, mc * 8);
+    t[n++] = MZH_PIN(z->h_hdr_off, mc * 8);
+    t[n++] = MZH_DEV(z->d_hdr_off, mc * 8);
+    t[n++] = MZH_PIN(z->h_blob_off, (mc + 1) * 4);
+    t[n++] = MZH_DEV(z->d_blob_off, (mc + 1) * 4);
+    t[n++] = MZH_PIN(z->h_blob, z->blob_cap + 16);
+    t[n++] = MZH_DEV(z->d_blob, z->blob_cap + 16);
+    t[n++] = MZH_DEV(z->d_region, z->region_cap);
+    t[n++] = MZH_PIN(z->h_region, z->region_cap);
+    t[n++] = MZH_PIN(z->h_salt, aes * mc * 16);
+    t[n++] = MZH_DEV(z->d_salt, aes * mc * 16);
+    t[n++] = MZH_PIN(z->h_keys, aes * mc * MZ_CUDA_WZAES_KEYREC);
+    t[n++] = MZH_DEV(z->d_keys, aes * mc * MZ_CUDA_WZAES_KEYREC);
+    t[n++] = MZH_DEV(z->d_pw, aes * 256);
+    t[n++] = MZH_PIN(z->h_mac, aes * mc * 20);
+    t[n++] = MZH_DEV(z->d_mac, aes * mc * 20);
+    t[n++] = MZH_PIN(z->h_coff, aes * mc * 8);
+    t[n++] = MZH_DEV(z->d_coff, aes * mc * 8);
+    t[n++] = MZH_PIN(z->h_clen, aes * mc * 8);
+    t[n++] = MZH_DEV(z->d_clen, aes * mc * 8);
+    return n;
+}
+
 static void za_free(za_slot *z) {
-    zc_free(&z->b);
+    mzh_piece t[ZA_PIECES];
+    mzh_free(t, za_pieces(z, t));
     if (z->stream)
         mz_cuda_stream_destroy(z->stream);
-    mz_cuda_host_free(z->h_out_len);
-    mz_cuda_host_free(z->h_dst_off);
-    mz_cuda_free(z->d_dst_off);
-    mz_cuda_host_free(z->h_hdr_off);
-    mz_cuda_free(z->d_hdr_off);
-    mz_cuda_host_free(z->h_blob_off);
-    mz_cuda_free(z->d_blob_off);
-    mz_cuda_host_free(z->h_blob);
-    mz_cuda_free(z->d_blob);
-    mz_cuda_free(z->d_region);
-    mz_cuda_host_free(z->h_region);
-    mz_cuda_host_free(z->h_salt);
-    mz_cuda_free(z->d_salt);
-    mz_cuda_host_free(z->h_keys);
-    mz_cuda_free(z->d_keys);
-    mz_cuda_free(z->d_pw);
-    mz_cuda_host_free(z->h_mac);
-    mz_cuda_free(z->d_mac);
-    mz_cuda_host_free(z->h_coff);
-    mz_cuda_free(z->d_coff);
-    mz_cuda_host_free(z->h_clen);
-    mz_cuda_free(z->d_clen);
     free(z->meta);
     memset(z, 0, sizeof(*z));
 }
 
-static int za_alloc(za_slot *z, size_t round_bytes, uint32_t max_chunks, size_t blob_cap, int aes) {
-    memset(z, 0, sizeof(*z));
-    z->has_aes = aes;
-    if (!zc_alloc(&z->b, round_bytes, max_chunks, 0))
+/* a new slot for the capacities and device set in *z */
+static int za_alloc(za_slot *z) {
+    mzh_piece t[ZA_PIECES];
+    const uint32_t max_chunks = z->b.max_chunks;
+    z->b.stride = mz_cuda_deflate_slot_bound(ZC_CHUNK);
+    z->region_cap = (size_t)max_chunks * z->b.stride + z->blob_cap + 64;
+    if (!mzh_alloc(t, za_pieces(z, t)))
         return 0;
-    z->blob_cap = blob_cap;
-    z->region_cap = (size_t)max_chunks * z->b.stride + blob_cap + 64;
-    z->h_out_len = (uint32_t *)mz_cuda_host_alloc((size_t)max_chunks * 4);
-    z->h_dst_off = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-    z->d_dst_off = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-    z->h_hdr_off = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-    z->d_hdr_off = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-    z->h_blob_off = (uint32_t *)mz_cuda_host_alloc(((size_t)max_chunks + 1) * 4);
-    z->d_blob_off = (uint32_t *)mz_cuda_malloc(((size_t)max_chunks + 1) * 4);
-    z->h_blob = (uint8_t *)mz_cuda_host_alloc(blob_cap + 16);
-    z->d_blob = (uint8_t *)mz_cuda_malloc(blob_cap + 16);
-    z->d_region = (uint8_t *)mz_cuda_malloc(z->region_cap);
-    z->h_region = (uint8_t *)mz_cuda_host_alloc(z->region_cap);
     z->meta = (za_meta *)malloc((size_t)max_chunks * sizeof(za_meta));
     z->stream = mz_cuda_stream_create();
-    if (aes) {
-        z->h_salt = (uint8_t *)mz_cuda_host_alloc((size_t)max_chunks * 16);
-        z->d_salt = (uint8_t *)mz_cuda_malloc((size_t)max_chunks * 16);
-        z->h_keys = (uint8_t *)mz_cuda_host_alloc((size_t)max_chunks * MZ_CUDA_WZAES_KEYREC);
-        z->d_keys = (uint8_t *)mz_cuda_malloc((size_t)max_chunks * MZ_CUDA_WZAES_KEYREC);
-        z->d_pw = (uint8_t *)mz_cuda_malloc(256);
-        z->h_mac = (uint8_t *)mz_cuda_host_alloc((size_t)max_chunks * 20);
-        z->d_mac = (uint8_t *)mz_cuda_malloc((size_t)max_chunks * 20);
-        z->h_coff = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-        z->d_coff = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-        z->h_clen = (uint64_t *)mz_cuda_host_alloc((size_t)max_chunks * 8);
-        z->d_clen = (uint64_t *)mz_cuda_malloc((size_t)max_chunks * 8);
-        if (!z->h_salt || !z->d_salt || !z->h_keys || !z->d_keys || !z->d_pw || !z->h_mac || !z->d_mac || !z->h_coff || !z->d_coff || !z->h_clen ||
-            !z->d_clen) {
-            za_free(z);
-            return 0;
-        }
-    }
-    if (!z->stream || !z->h_out_len || !z->h_dst_off || !z->d_dst_off || !z->h_hdr_off || !z->d_hdr_off || !z->h_blob_off || !z->d_blob_off || !z->h_blob ||
-        !z->d_blob || !z->d_region || !z->h_region || !z->meta) {
+    if (!z->meta || !z->stream) {
         za_free(z);
         return 0;
     }
     return 1;
 }
 
-/* Staging pool: a slot is ~130 MiB of page-locked and ~200 MiB of device memory, and making four of them costs more than half a
- * second -- as much as compressing 2 GiB. A process that writes archive after archive keeps up to eight idle slots (per device,
- * matched by capacity); MZ_CUDA_ZIP_POOL=0 turns the pool off, mz_zip_cuda_trim() empties it. */
-#define ZA_POOL_MAX 8
-static pthread_mutex_t g_za_mu = PTHREAD_MUTEX_INITIALIZER;
-static za_slot g_za_pool[ZA_POOL_MAX];
-static int g_za_n;
+/* One round of extraction on the device (K9 locate, K8, K9 stored copy, K5, K1, K7, K9 verify): the slot's staging, its CUDA
+ * stream, and the round in flight. Both extractors fill h_in and h_ent and call zr_run; mz_zip_cuda_extract_archive keeps up to
+ * four slots in flight on their own threads and pools them between calls (like the native writer's), mz_zip_cuda_extract_all
+ * runs one synchronously. mz_zip_cuda_extract_device and the reader carve the round arrays alone (zd_carve). */
+typedef struct zr_slot_s {
+    size_t in_cap, out_cap;
+    uint32_t max_ent;
+    int32_t device;
+    uint8_t *h_in, *d_in, *h_out, *d_out;
+    mz_cuda_zip_ent *h_ent, *d_ent;
+    uint8_t *h_sha, *d_sha;
+    uint32_t *h_status, *d_status;
+    mz_cuda_inflate_job *d_job;
+    mz_cuda_inflate_state *d_state;
+    uint64_t *d_seg_off, *d_seg_len64, *d_data_off, *d_coff, *d_clen;
+    uint32_t *d_seg_len, *d_residue, *d_crc;
+    uint8_t *d_digest, *d_salt, *d_keys, *d_pw, *d_mac;
+    void *stream;
+    /* the round in flight */
+    uint32_t first, last, n, njobs, nsha, na[4];
+    uint64_t max_clen[4];
+    size_t in_used, out_used;
+    const char *password;
+    int32_t err;
+    double gpu_ms;
+    pthread_t th;
+    int running;
+} zr_slot;
 
-static int za_pool_enabled(void) {
+#define ZR_ROUND_PIECES 16
+/* the arrays zr_launch uses for a round of m entries, digest_rows of them for K7's digests, into t; returns their number */
+static int zr_round_pieces(zr_slot *z, size_t m, size_t digest_rows, mzh_piece *t) {
+    int n = 0;
+    t[n++] = MZH_DEV(z->d_status, m * 4);
+    t[n++] = MZH_DEV(z->d_job, m * sizeof(mz_cuda_inflate_job));
+    t[n++] = MZH_DEV(z->d_state, m * sizeof(mz_cuda_inflate_state));
+    t[n++] = MZH_DEV(z->d_seg_off, m * 8);
+    t[n++] = MZH_DEV(z->d_seg_len64, m * 8);
+    t[n++] = MZH_DEV(z->d_data_off, m * 8);
+    t[n++] = MZH_DEV(z->d_coff, m * 8);
+    t[n++] = MZH_DEV(z->d_clen, m * 8);
+    t[n++] = MZH_DEV(z->d_seg_len, m * 4);
+    t[n++] = MZH_DEV(z->d_residue, m * 4);
+    t[n++] = MZH_DEV(z->d_crc, m * 4);
+    t[n++] = MZH_DEV(z->d_digest, digest_rows * 32);
+    t[n++] = MZH_DEV(z->d_salt, m * 16);
+    t[n++] = MZH_DEV(z->d_keys, m * MZ_CUDA_WZAES_KEYREC);
+    t[n++] = MZH_DEV(z->d_pw, 256);
+    t[n++] = MZH_DEV(z->d_mac, m * 20);
+    return n;
+}
+
+#define ZR_PIECES (9 + ZR_ROUND_PIECES)
+/* z's staging and round arrays for its capacities into t. in_cap: stored bytes of a round (+ 64 readable bytes past them); out_cap:
+ * plain bytes (+ 512); max_ent: entries */
+static int zr_pieces(zr_slot *z, mzh_piece *t) {
+    const size_t m = z->max_ent;
+    int n = 0;
+    t[n++] = MZH_PIN(z->h_in, z->in_cap + 64);
+    t[n++] = MZH_DEV(z->d_in, z->in_cap + 64);
+    t[n++] = MZH_PIN(z->h_out, z->out_cap + 512);
+    t[n++] = MZH_DEV(z->d_out, z->out_cap + 512);
+    t[n++] = MZH_PIN(z->h_ent, m * sizeof(mz_cuda_zip_ent));
+    t[n++] = MZH_DEV(z->d_ent, m * sizeof(mz_cuda_zip_ent));
+    t[n++] = MZH_PIN(z->h_sha, m * 32);
+    t[n++] = MZH_DEV(z->d_sha, m * 32);
+    t[n++] = MZH_PIN(z->h_status, m * 4);
+    return n + zr_round_pieces(z, m, m, t + n);
+}
+
+static void zr_free(zr_slot *z) {
+    mzh_piece t[ZR_PIECES];
+    mzh_free(t, zr_pieces(z, t));
+    if (z->stream)
+        mz_cuda_stream_destroy(z->stream);
+    memset(z, 0, sizeof(*z));
+}
+
+/* a new slot for the capacities set in *z, with its own stream or none (mz_zip_cuda_extract_all) */
+static int zr_alloc(zr_slot *z, int with_stream) {
+    mzh_piece t[ZR_PIECES];
+    if (!mzh_alloc(t, zr_pieces(z, t)))
+        return 0;
+    z->stream = with_stream ? mz_cuda_stream_create() : NULL;
+    if (with_stream && !z->stream) {
+        zr_free(z);
+        return 0;
+    }
+    return 1;
+}
+
+/* Staging pool: a writer slot is ~130 MiB of page-locked and ~200 MiB of device memory, and making four of them costs more than half
+ * a second -- as much as compressing 2 GiB. A process that writes or extracts archive after archive keeps up to eight idle slots of
+ * each kind, writer (za_slot) and extractor (zr_slot), per device and matched by capacity; MZ_CUDA_ZIP_POOL=0 turns the pool off,
+ * mz_zip_cuda_trim() empties it. */
+#define ZA_POOL_MAX 8
+enum { ZP_WRITER, ZP_EXTRACTOR };
+typedef union zp_slot_u {
+    za_slot w;
+    zr_slot x;
+} zp_slot;
+static pthread_mutex_t g_zp_mu = PTHREAD_MUTEX_INITIALIZER;
+static zp_slot g_zp[2][ZA_POOL_MAX];
+static int g_zp_n[2];
+
+static int zp_enabled(void) {
     const char *v = getenv("MZ_CUDA_ZIP_POOL");
     return !(v && v[0] == '0');
 }
 
-static int za_acquire(za_slot *z, int32_t dev, size_t round_bytes, uint32_t max_chunks, size_t blob_cap, int aes) {
+/* does the idle slot q serve the request r? Same device and capacities at least r's; a writer slot with the WinZip AES buffers
+ * serves a plain request, not the reverse */
+static int zp_serves(int kind, const zp_slot *q, const void *r) {
+    if (kind == ZP_WRITER) {
+        const za_slot *w = (const za_slot *)r;
+        return q->w.device == w->device && q->w.b.round_bytes >= w->b.round_bytes && q->w.b.max_chunks >= w->b.max_chunks &&
+               q->w.blob_cap >= w->blob_cap && (q->w.has_aes || !w->has_aes);
+    }
+    const zr_slot *x = (const zr_slot *)r;
+    return q->x.device == x->device && q->x.in_cap >= x->in_cap && q->x.out_cap >= x->out_cap && q->x.max_ent >= x->max_ent;
+}
+
+static void zp_free(int kind, void *z) {
+    if (kind == ZP_WRITER)
+        za_free((za_slot *)z);
+    else
+        zr_free((zr_slot *)z);
+}
+
+/* *z (a za_slot or zr_slot) holds the request: its device and capacities. An idle slot that serves it replaces it, with the round in
+ * flight cleared; else a new slot is made. 0 when that fails. */
+static int zp_acquire(int kind, void *z) {
+    const size_t size = kind == ZP_WRITER ? sizeof(za_slot) : sizeof(zr_slot);
     int hit = 0;
-    pthread_mutex_lock(&g_za_mu);
-    for (int i = 0; i < g_za_n; i++) {
-        const za_slot *q = &g_za_pool[i];
-        if (q->device == dev && q->b.round_bytes >= round_bytes && q->b.max_chunks >= max_chunks && q->blob_cap >= blob_cap && (q->has_aes || !aes)) {
-            *z = *q;
-            g_za_pool[i] = g_za_pool[--g_za_n];
-            hit = 1;
-            break;
+    pthread_mutex_lock(&g_zp_mu);
+    for (int i = 0; i < g_zp_n[kind] && !hit; i++) {
+        if ((hit = zp_serves(kind, &g_zp[kind][i], z))) {
+            memcpy(z, &g_zp[kind][i], size);
+            g_zp[kind][i] = g_zp[kind][--g_zp_n[kind]];
         }
     }
-    pthread_mutex_unlock(&g_za_mu);
-    if (hit) {
-        z->items = NULL;
-        z->first = z->last = z->nch = 0;
-        z->err = 0;
-        z->region_len = 0;
-        z->pack_ms = z->gpu_ms = 0;
-        z->running = 0;
-        z->password = NULL;
-        return 1;
+    pthread_mutex_unlock(&g_zp_mu);
+    if (!hit)
+        return kind == ZP_WRITER ? za_alloc((za_slot *)z) : zr_alloc((zr_slot *)z, 1);
+    if (kind == ZP_WRITER) {
+        za_slot *w = (za_slot *)z;
+        w->items = NULL;
+        w->first = w->last = w->nch = 0;
+        w->err = 0;
+        w->region_len = 0;
+        w->pack_ms = w->gpu_ms = 0;
+        w->running = 0;
+        w->password = NULL;
+    } else {
+        zr_slot *x = (zr_slot *)z;
+        x->running = 0;
+        x->err = 0;
     }
-    if (!za_alloc(z, round_bytes, max_chunks, blob_cap, aes))
-        return 0;
-    z->device = dev;
     return 1;
 }
 
-static void za_release(za_slot *z) {
+/* *z back to the pool, or freed: the pool is off or full, or z has no staging, or no stream (mz_zip_cuda_extract_all) */
+static void zp_release(int kind, void *z) {
+    const size_t size = kind == ZP_WRITER ? sizeof(za_slot) : sizeof(zr_slot);
+    const int whole = kind == ZP_WRITER ? ((za_slot *)z)->b.h_in != NULL : ((zr_slot *)z)->h_in && ((zr_slot *)z)->stream;
     int kept = 0;
-    if (z->b.h_in && za_pool_enabled()) {
-        pthread_mutex_lock(&g_za_mu);
-        if (g_za_n < ZA_POOL_MAX) {
-            g_za_pool[g_za_n++] = *z;
+    if (whole && zp_enabled()) {
+        pthread_mutex_lock(&g_zp_mu);
+        if (g_zp_n[kind] < ZA_POOL_MAX) {
+            memcpy(&g_zp[kind][g_zp_n[kind]++], z, size);
             kept = 1;
         }
-        pthread_mutex_unlock(&g_za_mu);
+        pthread_mutex_unlock(&g_zp_mu);
     }
     if (kept)
-        memset(z, 0, sizeof(*z));
+        memset(z, 0, size);
     else
-        za_free(z);
+        zp_free(kind, z);
 }
-
-static void zr_trim(void);
 
 void mz_zip_cuda_trim(void) {
     const int32_t dev0 = mz_cuda_get_device();
-    zr_trim();
-    pthread_mutex_lock(&g_za_mu);
-    for (int i = 0; i < g_za_n; i++) {
-        mz_cuda_set_device(g_za_pool[i].device);
-        za_free(&g_za_pool[i]);
+    pthread_mutex_lock(&g_zp_mu);
+    for (int kind = ZP_WRITER; kind <= ZP_EXTRACTOR; kind++) {
+        for (int i = 0; i < g_zp_n[kind]; i++) {
+            zp_slot *q = &g_zp[kind][i];
+            mz_cuda_set_device(kind == ZP_WRITER ? q->w.device : q->x.device);
+            zp_free(kind, q);
+        }
+        g_zp_n[kind] = 0;
     }
-    g_za_n = 0;
-    pthread_mutex_unlock(&g_za_mu);
+    pthread_mutex_unlock(&g_zp_mu);
     if (dev0 >= 0)
         mz_cuda_set_device(dev0);
 }
@@ -808,12 +888,7 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
         return MZ_SUPPORT_ERROR;
     /* 64 MiB rounds, four in preparation: each round's entries are packed into pinned staging by its own worker thread (that copy is
      * the slowest stage of a round), and small rounds keep the page-locked allocations -- and the time to make them -- small */
-    size_t round_bytes = 64u << 20;
-    {
-        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
-        if (v && atoll(v) > 0)
-            round_bytes = (size_t)atoll(v) << 20;
-    }
+    size_t round_bytes = mzh_round_bytes(64);
     size_t max_name = 0;
     for (uint32_t i = 0; i < count; i++) {
         if (!items[i].filename || items[i].size < 0 || (items[i].size > 0 && !items[i].data))
@@ -884,12 +959,16 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
         return MZ_MEM_ERROR;
     }
     for (uint32_t k = 0; k < nslots && err == MZ_OK; k++) {
-        const int32_t dev = ndev > 1 ? (int32_t)(k % (uint32_t)ndev) : dev0;
-        if (mz_cuda_set_device(dev) != MZ_OK || !za_acquire(&slots[k], dev, round_bytes, max_chunks + 1, max_blob, aes)) {
+        za_slot *z = &slots[k];
+        z->device = ndev > 1 ? (int32_t)(k % (uint32_t)ndev) : dev0;
+        z->b.round_bytes = round_bytes;
+        z->b.max_chunks = max_chunks + 1;
+        z->blob_cap = max_blob;
+        z->has_aes = aes;
+        if (mz_cuda_set_device(z->device) != MZ_OK || !zp_acquire(ZP_WRITER, z)) {
             err = MZ_MEM_ERROR;
             break;
         }
-        slots[k].device = dev;
         slots[k].items = items;
         slots[k].level = level;
         slots[k].flags = flags;
@@ -1024,7 +1103,7 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
     const double t_setup1 = now_ms();
     for (uint32_t k = 0; k < nslots; k++) {
         mz_cuda_set_device(slots[k].device);
-        za_release(&slots[k]);
+        zp_release(ZP_WRITER, &slots[k]);
     }
     mz_cuda_set_device(dev0);
     st.setup_ms += now_ms() - t_setup1;
@@ -1037,159 +1116,6 @@ int32_t mz_zip_cuda_write_archive_aes(void *base_stream, const mz_cuda_zip_item 
 }
 
 /* ---- batch extraction ------------------------------------------------------------------------------------------ */
-/* One round of extraction on the device (K9 locate, K8, K9 stored copy, K5, K1, K7, K9 verify): the slot's staging, its CUDA
- * stream, and the round in flight. Both extractors fill h_in and h_ent and call zr_run; mz_zip_cuda_extract_archive keeps up to
- * four slots in flight on their own threads and pools them between calls (like the native writer's), mz_zip_cuda_extract_all
- * runs one synchronously. */
-typedef struct zr_slot_s {
-    size_t in_cap, out_cap;
-    uint32_t max_ent;
-    int32_t device;
-    uint8_t *h_in, *d_in, *h_out, *d_out;
-    mz_cuda_zip_ent *h_ent, *d_ent;
-    uint8_t *h_sha, *d_sha;
-    uint32_t *h_status, *d_status;
-    mz_cuda_inflate_job *d_job;
-    mz_cuda_inflate_state *d_state;
-    uint64_t *d_seg_off, *d_seg_len64, *d_data_off, *d_coff, *d_clen;
-    uint32_t *d_seg_len, *d_residue, *d_crc;
-    uint8_t *d_digest, *d_salt, *d_keys, *d_pw, *d_mac;
-    void *stream;
-    /* the round in flight */
-    uint32_t first, last, n, njobs, nsha, na[4];
-    uint64_t max_clen[4];
-    size_t in_used, out_used;
-    const char *password;
-    int32_t err;
-    double gpu_ms;
-    pthread_t th;
-    int running;
-} zr_slot;
-
-static void zr_free(zr_slot *z) {
-    mz_cuda_host_free(z->h_in);
-    mz_cuda_free(z->d_in);
-    mz_cuda_host_free(z->h_out);
-    mz_cuda_free(z->d_out);
-    mz_cuda_host_free(z->h_ent);
-    mz_cuda_free(z->d_ent);
-    mz_cuda_host_free(z->h_sha);
-    mz_cuda_free(z->d_sha);
-    mz_cuda_host_free(z->h_status);
-    mz_cuda_free(z->d_status);
-    mz_cuda_free(z->d_job);
-    mz_cuda_free(z->d_state);
-    mz_cuda_free(z->d_seg_off);
-    mz_cuda_free(z->d_seg_len64);
-    mz_cuda_free(z->d_data_off);
-    mz_cuda_free(z->d_coff);
-    mz_cuda_free(z->d_clen);
-    mz_cuda_free(z->d_seg_len);
-    mz_cuda_free(z->d_residue);
-    mz_cuda_free(z->d_crc);
-    mz_cuda_free(z->d_digest);
-    mz_cuda_free(z->d_salt);
-    mz_cuda_free(z->d_keys);
-    mz_cuda_free(z->d_pw);
-    mz_cuda_free(z->d_mac);
-    if (z->stream)
-        mz_cuda_stream_destroy(z->stream);
-    memset(z, 0, sizeof(*z));
-}
-
-/* in_cap: stored bytes of a round (+ 64 readable bytes past them); out_cap: plain bytes (+ 512); max_ent: entries */
-static int zr_alloc(zr_slot *z, size_t in_cap, size_t out_cap, uint32_t max_ent, int with_stream) {
-    const size_t n = max_ent;
-    memset(z, 0, sizeof(*z));
-    z->in_cap = in_cap;
-    z->out_cap = out_cap;
-    z->max_ent = max_ent;
-    z->h_in = (uint8_t *)mz_cuda_host_alloc(in_cap + 64);
-    z->d_in = (uint8_t *)mz_cuda_malloc(in_cap + 64);
-    z->h_out = (uint8_t *)mz_cuda_host_alloc(out_cap + 512);
-    z->d_out = (uint8_t *)mz_cuda_malloc(out_cap + 512);
-    z->h_ent = (mz_cuda_zip_ent *)mz_cuda_host_alloc(n * sizeof(mz_cuda_zip_ent));
-    z->d_ent = (mz_cuda_zip_ent *)mz_cuda_malloc(n * sizeof(mz_cuda_zip_ent));
-    z->h_sha = (uint8_t *)mz_cuda_host_alloc(n * 32);
-    z->d_sha = (uint8_t *)mz_cuda_malloc(n * 32);
-    z->h_status = (uint32_t *)mz_cuda_host_alloc(n * 4);
-    z->d_status = (uint32_t *)mz_cuda_malloc(n * 4);
-    z->d_job = (mz_cuda_inflate_job *)mz_cuda_malloc(n * sizeof(mz_cuda_inflate_job));
-    z->d_state = (mz_cuda_inflate_state *)mz_cuda_malloc(n * sizeof(mz_cuda_inflate_state));
-    z->d_seg_off = (uint64_t *)mz_cuda_malloc(n * 8);
-    z->d_seg_len64 = (uint64_t *)mz_cuda_malloc(n * 8);
-    z->d_data_off = (uint64_t *)mz_cuda_malloc(n * 8);
-    z->d_coff = (uint64_t *)mz_cuda_malloc(n * 8);
-    z->d_clen = (uint64_t *)mz_cuda_malloc(n * 8);
-    z->d_seg_len = (uint32_t *)mz_cuda_malloc(n * 4);
-    z->d_residue = (uint32_t *)mz_cuda_malloc(n * 4);
-    z->d_crc = (uint32_t *)mz_cuda_malloc(n * 4);
-    z->d_digest = (uint8_t *)mz_cuda_malloc(n * 32);
-    z->d_salt = (uint8_t *)mz_cuda_malloc(n * 16);
-    z->d_keys = (uint8_t *)mz_cuda_malloc(n * MZ_CUDA_WZAES_KEYREC);
-    z->d_pw = (uint8_t *)mz_cuda_malloc(256);
-    z->d_mac = (uint8_t *)mz_cuda_malloc(n * 20);
-    z->stream = with_stream ? mz_cuda_stream_create() : NULL;
-    if (!z->h_in || !z->d_in || !z->h_out || !z->d_out || !z->h_ent || !z->d_ent || !z->h_sha || !z->d_sha || !z->h_status || !z->d_status ||
-        !z->d_job || !z->d_state || !z->d_seg_off || !z->d_seg_len64 || !z->d_data_off || !z->d_coff || !z->d_clen || !z->d_seg_len ||
-        !z->d_residue || !z->d_crc || !z->d_digest || !z->d_salt || !z->d_keys || !z->d_pw || !z->d_mac || (with_stream && !z->stream)) {
-        zr_free(z);
-        return 0;
-    }
-    return 1;
-}
-
-/* the extractor's staging pool: same rules as the writer's (MZ_CUDA_ZIP_POOL=0 off, mz_zip_cuda_trim() empties it) */
-static zr_slot g_zr_pool[ZA_POOL_MAX];
-static int g_zr_n;
-
-static void zr_trim(void) {
-    pthread_mutex_lock(&g_za_mu);
-    for (int i = 0; i < g_zr_n; i++) {
-        mz_cuda_set_device(g_zr_pool[i].device);
-        zr_free(&g_zr_pool[i]);
-    }
-    g_zr_n = 0;
-    pthread_mutex_unlock(&g_za_mu);
-}
-
-static int zr_acquire(zr_slot *z, int32_t dev, size_t in_cap, size_t out_cap, uint32_t max_ent) {
-    int hit = 0;
-    pthread_mutex_lock(&g_za_mu);
-    for (int i = 0; i < g_zr_n; i++) {
-        const zr_slot *q = &g_zr_pool[i];
-        if (q->device == dev && q->in_cap >= in_cap && q->out_cap >= out_cap && q->max_ent >= max_ent) {
-            *z = *q;
-            g_zr_pool[i] = g_zr_pool[--g_zr_n];
-            hit = 1;
-            break;
-        }
-    }
-    pthread_mutex_unlock(&g_za_mu);
-    if (!hit && !zr_alloc(z, in_cap, out_cap, max_ent, 1))
-        return 0;
-    z->device = dev;
-    z->running = 0;
-    z->err = 0;
-    return 1;
-}
-
-static void zr_release(zr_slot *z) {
-    int kept = 0;
-    if (z->h_in && z->stream && za_pool_enabled()) {
-        pthread_mutex_lock(&g_za_mu);
-        if (g_zr_n < ZA_POOL_MAX) {
-            g_zr_pool[g_zr_n++] = *z;
-            kept = 1;
-        }
-        pthread_mutex_unlock(&g_za_mu);
-    }
-    if (kept)
-        memset(z, 0, sizeof(*z));
-    else
-        zr_free(z);
-}
-
 /* the round's launches on stream s, from the K9 table in z->d_ent (and digests in z->d_sha) over the stored bytes buf[0, buf_len)
  * (32 readable bytes past them) into out: locate, K8 per strength (decrypts buf in place), stored copy, K5, K1, K7, verify */
 static int32_t zr_launch(zr_slot *z, uint8_t *buf, uint64_t buf_len, uint8_t *out, void *s) {
@@ -1419,19 +1345,16 @@ int32_t mz_zip_cuda_extract_all_aes(void *zip_handle, const char *password, mz_c
         return MZ_PARAM_ERROR;
     if (mzh_gpu_required("mz_zip_cuda"))
         return MZ_SUPPORT_ERROR;
-    size_t comp_cap = 128u << 20, out_cap = 512u << 20;
-    {
-        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
-        if (v && atoll(v) > 0) {
-            comp_cap = (size_t)atoll(v) << 20;
-            out_cap = comp_cap * 4;
-        }
-    }
+    const size_t comp_cap = mzh_round_bytes(128), out_cap = comp_cap * 4;
     const uint32_t max_entries = 65536;
     const size_t names_cap = (size_t)max_entries * 64;
     zx_entry *ent = (zx_entry *)malloc((size_t)max_entries * sizeof(zx_entry));
     char *names = (char *)malloc(names_cap);
-    if (!ent || !names || !zr_alloc(&z, comp_cap, out_cap, max_entries, 0)) {
+    memset(&z, 0, sizeof(z));
+    z.in_cap = comp_cap;
+    z.out_cap = out_cap;
+    z.max_ent = max_entries;
+    if (!ent || !names || !zr_alloc(&z, 0)) {
         free(ent);
         free(names);
         return MZ_MEM_ERROR;
@@ -1815,12 +1738,7 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
     }
     /* rounds: runs of entries in directory order whose extents fit the staging (32 MiB by default) and whose plain bytes fit four
      * times that; an entry larger than a round gets a round of its own size */
-    size_t round_bytes = 32u << 20;
-    {
-        const char *v = getenv("MZ_CUDA_ZIP_ROUND_MB");
-        if (v && atoll(v) > 0)
-            round_bytes = (size_t)atoll(v) << 20;
-    }
+    const size_t round_bytes = mzh_round_bytes(32);
     const size_t out_round = round_bytes * 4;
     uint32_t nrounds = 0, rcap = 16, max_ent = 1;
     size_t max_in = 64, max_out = 64;
@@ -1881,10 +1799,14 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
     if (err == MZ_OK && !slots)
         err = MZ_MEM_ERROR;
     for (uint32_t k = 0; k < nslots && err == MZ_OK && nrounds; k++) {
-        const int32_t dev = ndev > 1 ? (int32_t)(k % (uint32_t)ndev) : dev0;
-        if (mz_cuda_set_device(dev) != MZ_OK || !zr_acquire(&slots[k], dev, max_in, max_out, max_ent))
+        zr_slot *z = &slots[k];
+        z->device = ndev > 1 ? (int32_t)(k % (uint32_t)ndev) : dev0;
+        z->in_cap = max_in;
+        z->out_cap = max_out;
+        z->max_ent = max_ent;
+        if (mz_cuda_set_device(z->device) != MZ_OK || !zp_acquire(ZP_EXTRACTOR, z))
             err = MZ_MEM_ERROR;
-        slots[k].password = password;
+        z->password = password;
     }
     mz_cuda_set_device(dev0);
     st.setup_ms = now_ms() - t_setup0;
@@ -1946,7 +1868,7 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
         if (oversized)
             zr_free(&slots[k]);
         else
-            zr_release(&slots[k]);
+            zp_release(ZP_EXTRACTOR, &slots[k]);
     }
     mz_cuda_set_device(dev0);
     st.setup_ms += now_ms() - t_setup1;
@@ -1961,17 +1883,13 @@ int32_t mz_zip_cuda_extract_archive(void *base_stream, const char *password, uin
 }
 
 /* ---- an archive in device memory (mz_zip_cuda_extract_device) ------------------------------------------------------------ */
-/* the round arrays K9 / K8 / K5 / K1 / K7 need for n entries, and the first-failure word, carved from one device allocation (returned;
- * NULL when it fails). The K9 table and the digests come from the directory parse. */
-static uint8_t *zd_carve(zr_slot *z, uint32_t n, uint32_t **first) {
-    const size_t m = n ? n : 1;
-    const size_t sz[17] = {m * 4, m * sizeof(mz_cuda_inflate_job), m * sizeof(mz_cuda_inflate_state), m * 8, m * 8, m * 8, m * 8, m * 8, m * 4,
-                           m * 4, m * 4, z->nsha ? m * 32 : 32, m * 16, m * MZ_CUDA_WZAES_KEYREC, 256, m * 20, 4};
-    void **out[17] = {(void **)&z->d_status, (void **)&z->d_job, (void **)&z->d_state, (void **)&z->d_seg_off, (void **)&z->d_seg_len64,
-                      (void **)&z->d_data_off, (void **)&z->d_coff, (void **)&z->d_clen, (void **)&z->d_seg_len, (void **)&z->d_residue,
-                      (void **)&z->d_crc, (void **)&z->d_digest, (void **)&z->d_salt, (void **)&z->d_keys, (void **)&z->d_pw, (void **)&z->d_mac,
-                      (void **)first};
-    return mzh_carve(sz, out, 17);
+/* zr_launch's arrays for a round of n entries (digest_rows of them for the digests), and the first-failure word, carved from one
+ * device allocation (returned; NULL when it fails). The K9 table and the expected digests come from the directory parse. */
+static uint8_t *zd_carve(zr_slot *z, uint32_t n, size_t digest_rows, uint32_t **first) {
+    mzh_piece t[ZR_ROUND_PIECES + 1];
+    const int k = zr_round_pieces(z, n ? n : 1, digest_rows, t);
+    t[k] = MZH_DEV(*first, 4);
+    return mzh_carve(t, k + 1);
 }
 
 int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const char *password, mz_cuda_zip_dev_entry *d_entries, uint32_t max_entries,
@@ -2029,7 +1947,7 @@ int32_t mz_zip_cuda_extract_device(const void *d_archive, uint64_t len, const ch
         const int aes = dir.na[1] || dir.na[2] || dir.na[3];
         uint8_t *buf = (uint8_t *)d_archive, *copy = NULL;
         uint32_t *d_first = NULL;
-        uint8_t *work = zd_carve(&z, dir.count, &d_first);
+        uint8_t *work = zd_carve(&z, dir.count, dir.nsha ? dir.count : 1, &d_first);
         if (!work || (aes && !(copy = (uint8_t *)mz_cuda_malloc(dir.cd_off + 32))))
             err = MZ_MEM_ERROR;
         st.setup_ms = now_ms() - t1;
@@ -2114,14 +2032,13 @@ static int32_t zu_reserve(mz_zip_cuda_dev_reader *r, uint32_t n) {
     r->work = r->selw = NULL;
     r->cap = 0;
     uint32_t *unused;
-    r->z.nsha = 1; /* zd_carve: a digest row per slot */
-    r->work = zd_carve(&r->z, (uint32_t)cap, &unused);
     const size_t m = (size_t)cap;
-    const size_t sz[5] = {m * sizeof(mz_cuda_zip_sel_count), (m + 1) * sizeof(mz_cuda_zip_sel_count),
-                          (m / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_sel_count), m * sizeof(mz_cuda_zip_ent), 8};
-    void **out[5] = {(void **)&r->cnt, (void **)&r->pre, &r->part, (void **)&r->sel, (void **)&r->first};
+    r->work = zd_carve(&r->z, (uint32_t)cap, m, &unused);
+    const mzh_piece t[5] = {MZH_DEV(r->cnt, m * sizeof(mz_cuda_zip_sel_count)), MZH_DEV(r->pre, (m + 1) * sizeof(mz_cuda_zip_sel_count)),
+                            MZH_DEV(r->part, (m / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_sel_count)),
+                            MZH_DEV(r->sel, m * sizeof(mz_cuda_zip_ent)), MZH_DEV(r->first, 8)};
     if (r->work)
-        r->selw = mzh_carve(sz, out, 5);
+        r->selw = mzh_carve(t, 5);
     if (!r->work || !r->selw) {
         mz_cuda_free(r->work);
         r->work = NULL;
@@ -2407,10 +2324,10 @@ static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_nam
     w.n_base = f->n;
     const size_t m = (size_t)count + 1, tiles = (size_t)count / MZ_CUDA_ZIP_WR_TILE + 1;
     /* 1. validation and per-item counts: the first invalid item and the totals come back */
-    const size_t sz1[4] = {16, m * sizeof(mz_cuda_zip_wr_count), m * sizeof(mz_cuda_zip_wr_count), tiles * sizeof(mz_cuda_zip_wr_count)};
-    void **p1[4] = {(void **)&w.bad, (void **)&w.cnt, (void **)&w.pre, &w.part};
+    const mzh_piece p1[4] = {MZH_DEV(w.bad, 16), MZH_DEV(w.cnt, m * sizeof(mz_cuda_zip_wr_count)), MZH_DEV(w.pre, m * sizeof(mz_cuda_zip_wr_count)),
+                             MZH_DEV(w.part, tiles * sizeof(mz_cuda_zip_wr_count))};
     double ts = now_ms();
-    uint8_t *work1 = mzh_carve(sz1, p1, 4), *work2 = NULL;
+    uint8_t *work1 = mzh_carve(p1, 4), *work2 = NULL;
     st.setup_ms += now_ms() - ts;
     if (!work1) {
         *stats_out = st;
@@ -2448,18 +2365,18 @@ static int32_t zw_write(const zw_front *f, const void *d_data, const void *d_nam
     const size_t ptiles = ((size_t)R > n ? (size_t)R : n) / MZ_CUDA_ZIP_WR_TILE + 1;
     uint8_t *slots = NULL, *pw = NULL;
     void *digest = NULL, *salt = NULL, *keys = NULL, *mac = NULL;
-    const size_t sz2[26] = {nch * 8, nch * 4, nch, nch * 4, nch * 4, nch * 4, nch * 4, (nch + 1) * 8, nch * 8,
-                            n * 8, n * 8, n * 8, (n + 1) * 8, n * 8, n * 8, n * 8, n * 4, 8, ptiles * sizeof(mz_cuda_zip_wr_count),
-                            (size_t)R * stride, w.sha ? n * 32 : 32, aes ? n * 16 : 16, aes ? n * MZ_CUDA_WZAES_KEYREC : 16, aes ? n * 20 : 16, 256,
-                            16};
     void *part2 = NULL, *spare = NULL;
-    void **p2[26] = {(void **)&w.c_off, (void **)&w.c_len, (void **)&w.c_flags, (void **)&w.c_item, (void **)&w.out_len, (void **)&w.residue, (void **)&w.glen,
-                     (void **)&w.S, (void **)&w.dst, (void **)&w.e_lh, (void **)&w.e_csize, (void **)&w.e_cd, (void **)&w.e_cdpre, (void **)&w.e_coff,
-                     (void **)&w.e_off, (void **)&w.e_len, (void **)&w.e_crc, (void **)&w.max_csize, &part2, (void **)&slots, &digest, &salt, &keys, &mac,
-                     (void **)&pw, &spare};
+    const mzh_piece p2[26] = {MZH_DEV(w.c_off, nch * 8), MZH_DEV(w.c_len, nch * 4), MZH_DEV(w.c_flags, nch), MZH_DEV(w.c_item, nch * 4),
+                              MZH_DEV(w.out_len, nch * 4), MZH_DEV(w.residue, nch * 4), MZH_DEV(w.glen, nch * 4), MZH_DEV(w.S, (nch + 1) * 8),
+                              MZH_DEV(w.dst, nch * 8), MZH_DEV(w.e_lh, n * 8), MZH_DEV(w.e_csize, n * 8), MZH_DEV(w.e_cd, n * 8),
+                              MZH_DEV(w.e_cdpre, (n + 1) * 8), MZH_DEV(w.e_coff, n * 8), MZH_DEV(w.e_off, n * 8), MZH_DEV(w.e_len, n * 8),
+                              MZH_DEV(w.e_crc, n * 4), MZH_DEV(w.max_csize, 8), MZH_DEV(part2, ptiles * sizeof(mz_cuda_zip_wr_count)),
+                              MZH_DEV(slots, (size_t)R * stride), MZH_DEV(digest, w.sha ? n * 32 : 32), MZH_DEV(salt, aes ? n * 16 : 16),
+                              MZH_DEV(keys, aes ? n * MZ_CUDA_WZAES_KEYREC : 16), MZH_DEV(mac, aes ? n * 20 : 16), MZH_DEV(pw, 256),
+                              MZH_DEV(spare, 16)};
     ts = now_ms();
     if (!err)
-        work2 = mzh_carve(sz2, p2, 26);
+        work2 = mzh_carve(p2, 26);
     st.setup_ms += now_ms() - ts;
     if (!err && !work2)
         err = MZ_MEM_ERROR;
@@ -2647,11 +2564,11 @@ int32_t mz_zip_cuda_update_device(const void *d_src, uint64_t src_len, const uin
     uint8_t *work = NULL;
     if (!err) {
         const size_t m = (size_t)n + 1;
-        const size_t sz[4] = {m * sizeof(mz_cuda_zip_up_count), m * sizeof(mz_cuda_zip_up_count),
-                              ((size_t)n / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_up_count), 8 * MZ_CUDA_ZIP_UP_INFO};
-        void **p[4] = {(void **)&u->cnt, (void **)&u->pre, &u->part, (void **)&u->info};
+        const mzh_piece t[4] = {MZH_DEV(u->cnt, m * sizeof(mz_cuda_zip_up_count)), MZH_DEV(u->pre, m * sizeof(mz_cuda_zip_up_count)),
+                                MZH_DEV(u->part, ((size_t)n / MZ_CUDA_ZIP_WR_TILE + 1) * sizeof(mz_cuda_zip_up_count)),
+                                MZH_DEV(u->info, 8 * MZ_CUDA_ZIP_UP_INFO)};
         const double ts = now_ms();
-        work = mzh_carve(sz, p, 4);
+        work = mzh_carve(t, 4);
         st.setup_ms += now_ms() - ts;
         if (!work)
             err = MZ_MEM_ERROR;
