@@ -227,10 +227,25 @@ __device__ __noinline__ int inf_slow_decode(uint32_t bits, const uint16_t *count
     return -1;
 }
 
+/* An incomplete set (zlib allows one code of length 1, and no distance code at all) leaves 1-bit patterns without a symbol:
+ * mark them invalid with their bit, as zlib's tables do, so that decoding one consumes that bit and a truncated stream is told
+ * from a corrupt one. l1 / l2: what inf_build returned for the literal/length and the distance set. Warp-cooperative. */
+__device__ __forceinline__ void inf_mark_invalid(InfTables &T, int l1, int l2) {
+    const unsigned lane = lane_id();
+    if (l1 > 0)
+        for (int i = (int)lane; i < (1 << INF_PB); i += 32)
+            if (T.lit[i] == 0) T.lit[i] = 1u | (INF_K_BAD << 8);
+    if (l2 > 0)
+        for (int i = (int)lane; i < (1 << INF_DB); i += 32)
+            if (T.dist[i] == 0) T.dist[i] = 1u | (INF_K_BAD << 8);
+    __syncwarp();
+}
+
 /* Warp-cooperative: read a dynamic block header (the bits after BFINAL/BTYPE) and build both decode tables
  * (RFC1951 3.2.7; zlib's rules for incomplete sets). EVERY lane runs the same bit reader over the same bits
  * (uniform control flow, no broadcasts); shared memory is written by lane 0 or by lanes in parallel.
- * Returns 0 or an INF_ST_* error (the same in all lanes). */
+ * Returns 0 or an INF_ST_* error (the same in all lanes). Every check comes after all the bits it depends on, as
+ * zlib's NEEDBITS does: a check that failed on bits past the input's end is a truncation, which the state save tells. */
 __device__ __forceinline__ int inf_dynamic_header(InfBits &b, InfTables &T, uint32_t &nlit, uint32_t &ndist) {
     const unsigned lane = lane_id();
     nlit = b.get(5) + 257;
@@ -272,12 +287,11 @@ __device__ __forceinline__ int inf_dynamic_header(InfBits &b, InfTables &T, uint
             } else {
                 uint32_t rep, val = 0;
                 if (sym == 16) {
-                    if (idx == 0) return INF_ST_DATA_ERROR;
                     val = prev;
                     rep = 3 + b.get(2);
                 } else if (sym == 17) rep = 3 + b.get(3);
                 else rep = 11 + b.get(7);
-                if (idx + rep > total) return INF_ST_DATA_ERROR;
+                if ((sym == 16 && idx == 0) || idx + rep > total) return INF_ST_DATA_ERROR; /* after the extra bits */
                 for (uint32_t r = lane; r < rep; r += 32) lens[idx + r] = (uint8_t)val;
                 idx += rep;
                 prev = val;
@@ -307,6 +321,7 @@ __device__ __forceinline__ int inf_dynamic_header(InfBits &b, InfTables &T, uint
     uint32_t usedl = nlit - T.lcount[0], usedd = ndist - T.dcount[0];
     if (l1 < 0 || l2 < 0 || (l1 > 0 && !(usedl == 1 && T.lcount[1] == 1)) || (l2 > 0 && usedd != 0 && !(usedd == 1 && T.dcount[1] == 1)))
         return INF_ST_DATA_ERROR;
+    inf_mark_invalid(T, l1, l2);
     return 0;
 }
 
@@ -468,9 +483,10 @@ __device__ __forceinline__ void inf_decode_window(const InflateJob &job, Inflate
     if (phase == INF_PH_CODES) { /* resume inside a Huffman block: rebuild the tables */
         for (int i = (int)lane; i < 320; i += 32) T.lens[i] = st->lens[i];
         __syncwarp();
-        inf_build(T.lens, (int)nlit, T.lcount, T.lsym, T.lit, INF_PB, INF_ALPHA_LITLEN, T.scratch);
-        inf_build(T.lens + nlit, (int)ndist, T.dcount, T.dsym, T.dist, INF_DB, INF_ALPHA_DIST, T.scratch);
+        const int l1 = inf_build(T.lens, (int)nlit, T.lcount, T.lsym, T.lit, INF_PB, INF_ALPHA_LITLEN, T.scratch);
+        const int l2 = inf_build(T.lens + nlit, (int)ndist, T.dcount, T.dsym, T.dist, INF_DB, INF_ALPHA_DIST, T.scratch);
         __syncwarp();
+        inf_mark_invalid(T, l1, l2);
     }
     while (status == INF_ST_RUN && why == INF_WHY_NONE) {
         if (phase == INF_PH_HEADER) {
@@ -490,11 +506,11 @@ __device__ __forceinline__ void inf_decode_window(const InflateJob &job, Inflate
             } else if (type == 1) {
                 __syncwarp();
                 for (int i = (int)lane; i < 288; i += 32) T.lens[i] = i < 144 ? 8 : (i < 256 ? 9 : (i < 280 ? 7 : 8));
-                if (lane < 30) T.lens[288 + lane] = 5;
-                nlit = 288; ndist = 30;
+                T.lens[288 + lane] = 5; /* 32 distance codes: 30 and 31 decode (all 5 bits) as invalid, as in zlib */
+                nlit = 288; ndist = 32;
                 __syncwarp();
                 inf_build(T.lens, 288, T.lcount, T.lsym, T.lit, INF_PB, INF_ALPHA_LITLEN, T.scratch);
-                inf_build(T.lens + 288, 30, T.dcount, T.dsym, T.dist, INF_DB, INF_ALPHA_DIST, T.scratch);
+                inf_build(T.lens + 288, 32, T.dcount, T.dsym, T.dist, INF_DB, INF_ALPHA_DIST, T.scratch);
                 __syncwarp();
                 phase = INF_PH_CODES;
             } else if (type == 2) {
@@ -616,6 +632,10 @@ __device__ __forceinline__ void inf_decode_window(const InflateJob &job, Inflate
     if (lane == 0) {
         uint64_t bp = b.bitpos();
         if (status == INF_ST_END) bp = (bp + 7) & ~7ull; /* the partial last byte is consumed */
+        if (bp > b.avail_bits) { /* the decoder read past the input's end: a truncated stream, whatever those bits made it decide */
+            bp = b.avail_bits;
+            if (status < 0) status = INF_ST_BUF_ERROR;
+        }
         st->in_bitpos = job.in_base * 8 + bp;
         st->out_pos = out_pos;
         st->status = status;

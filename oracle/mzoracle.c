@@ -264,8 +264,8 @@ static int build_fixed(orc_huff *lit, orc_huff *dist) {
     for (; i < 280; i++) lens[i] = 7;
     for (; i < 288; i++) lens[i] = 8;
     huff_build(lit, lens, 288);
-    for (i = 0; i < 30; i++) lens[i] = 5;
-    huff_build(dist, lens, 30);
+    for (i = 0; i < 32; i++) lens[i] = 5; /* codes 30 and 31 exist and are invalid when decoded, as in zlib */
+    huff_build(dist, lens, 32);
     return 0;
 }
 
@@ -299,9 +299,7 @@ static int read_dynamic(orc_state *s, orc_huff *lit, orc_huff *dist) {
         } else {
             int rep, val = 0;
             if (sym == 16) {
-                if (idx == 0)
-                    return ORC_DATA_ERROR;
-                val = lens[idx - 1];
+                val = idx ? lens[idx - 1] : 0;
                 rep = 3 + (int)get_bits(s, 2);
             } else if (sym == 17) {
                 rep = 3 + (int)get_bits(s, 3);
@@ -309,8 +307,8 @@ static int read_dynamic(orc_state *s, orc_huff *lit, orc_huff *dist) {
                 rep = 11 + (int)get_bits(s, 7);
             }
             if (s->starved)
-                return ORC_BUF_ERROR;
-            if (idx + rep > nlen + ndist)
+                return ORC_BUF_ERROR; /* zlib decides on a repeat once its extra bits are in */
+            if ((sym == 16 && idx == 0) || idx + rep > nlen + ndist)
                 return ORC_DATA_ERROR;
             while (rep--)
                 lens[idx++] = (uint8_t)val;
@@ -319,10 +317,10 @@ static int read_dynamic(orc_state *s, orc_huff *lit, orc_huff *dist) {
     if (lens[256] == 0)
         return ORC_DATA_ERROR; /* no end-of-block code */
     int err = huff_build(lit, lens, nlen);
-    if (err < 0 || (err > 0 && nlen - lit->count[0] != 1))
-        return ORC_DATA_ERROR; /* incomplete only allowed for a single code */
+    if (err < 0 || (err > 0 && !(nlen - lit->count[0] == 1 && lit->count[1] == 1)))
+        return ORC_DATA_ERROR; /* incomplete only allowed for a single code of length 1 */
     err = huff_build(dist, lens + nlen, ndist);
-    if (err < 0 || (err > 0 && ndist - dist->count[0] != 1))
+    if (err < 0 || (err > 0 && !(ndist - dist->count[0] == 1 && dist->count[1] == 1)))
         return ORC_DATA_ERROR;
     return ORC_OK;
 }
