@@ -30,8 +30,8 @@
  *              into the staging buffer (aliases the hash table). The block's total comes from the histograms in D, so whether
  *              the block is stored is known before this pass
  *   G flush    staging -> global in 16-byte units; partial tail carried into the next block
- * Blocks that would not shrink are emitted as stored blocks. A unit with more entries than the list
- * holds is coded as two blocks (batch halves). A non-final chunk ends with an empty stored block
+ * Every unit is coded as exactly one block: a dynamic one, or a stored one where the dynamic block would not be
+ * smaller. A non-final chunk ends with an empty stored block
  * (00 00 FF FF after bit padding) so chunks join byte-wise; the final chunk carries BFINAL.
  */
 #ifndef MZ_DEFLATE_KERNEL_CUH
@@ -1252,6 +1252,9 @@ __global__ void __launch_bounds__(DF_THREADS, HIST ? 1 : 2) deflate_chunks_kerne
                 /* ---- D: codes (10 warps on a named barrier; the rest wait here) ------------------------- */
 #ifdef MZ_DF_CODES_HOOK /* test builds only (tests/emu/emu_df_codes.cc): record the histograms the builder is given */
                 if (tid == 0) MZ_DF_CODES_HOOK(s_hist_ll, (const uint32_t *)(smem + DF_OFF_HIST2), s_hist_d);
+#endif
+#ifdef MZ_DF_UNIT_HOOK /* ... and which chunk and unit each one belongs to */
+                if (tid == 0) MZ_DF_UNIT_HOOK(chunk, u);
 #endif
                 if (tid < DF_BB_THREADS)
                     block_build_codes(s_hist_ll, (const uint32_t *)(smem + DF_OFF_HIST2), s_hist_d, s_lens_ll, s_lens_d, s_code_ll, s_code_d, s_bits_ll, s_bits_d, s_bb,
